@@ -14,10 +14,10 @@ N > 1 (torchrun, one rank per GPU): the default is north_star's split -- ONE 80-
 exchange steps are NCCL all-gathers over NVLink; BASELINE config[2] (240 frames, subvideo_length 80, same sharding) is
 reported alongside as `config2_240f`.  `--mode weak` runs one independent subvideo per GPU instead.
 
-`--impl reference` times the UNMODIFIED reference (installed by __graft_entry__.build() into baseline/_ref, which is
-git-ignored but travels to the GPU box) on the host cores: one pass over the first 16 frames of the same clip, all
-threads; it also reports the reference's own PyTorch-CUDA fp16 path on the same B200 at the full 80 frames
-(`reference_cuda`, the number SURVEY.md 8d calls "the number to beat").  Without baseline/_ref it falls back to the
+`--impl reference` times the UNMODIFIED reference, installed by __graft_entry__.build() into the git-ignored
+oracle/_ref (oracle/build_ref.py), on the host cores: one pass over the first 16 frames of the same clip, all
+threads; it also reports the reference's own PyTorch-CUDA fp16 path on the same GPU at the full 80 frames
+(`reference_cuda`, the number SURVEY.md 8d calls "the number to beat").  Without oracle/_ref it falls back to the
 CPU oracle port.
 """
 import argparse
@@ -52,7 +52,7 @@ PARAMS = dict(mask_dilates=5, flow_mask_dilates=8, ref_stride=10, neighbor_lengt
               fp16="enable")
 METRIC = "inpainted frames/sec at 640x360, 80-frame subvideo"
 WORKLOAD = "configs[1]: 80-frame 640x360 synthetic clip, ref_stride=10 neighbor_length=10 raft_iter=20 fp16"
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")   # oracle/build_ref.py, run by __graft_entry__.build()
 
 
 def peaks():
@@ -61,7 +61,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor_burst=d["bf16_tflops"], tensor=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor=1400.0, source="fallback")
+    # NVIDIA data sheet, H100 SXM at 700 W: HBM3 3.35 TB/s, dense BF16/FP16 989 TFLOP/s (not reached figures)
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor=989.0, source="H100 SXM data sheet")
 
 
 def ncu_traffic():
@@ -110,16 +111,16 @@ def synthetic_state_dicts():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# the reference itself (baseline/_ref) and, when it is absent, the CPU oracle port
+# the reference itself (oracle/_ref) and, when it is absent, the CPU oracle port
 # ------------------------------------------------------------------------------------------------------------------
 def host_threads():
-    """Threads of the CPU arm: every host core up to PP_CPU_THREADS (default 32 -- beyond that the 1/8-resolution
-    convolutions of the recurrent stages stop scaling on the 128-core host, profiles/r01_cpu_threads.log)."""
+    """Threads of the CPU arm: every host core up to PP_CPU_THREADS (default 32: the 1/8-resolution convolutions of
+    the recurrent stages are small, so more threads mostly add synchronisation)."""
     return min(os.cpu_count() or 1, int(os.environ.get("PP_CPU_THREADS", 32)))
 
 
 def load_reference():
-    """Import the unmodified reference package from baseline/_ref with a stub ``comfy.model_management`` (the one
+    """Import the unmodified reference package from oracle/_ref with a stub ``comfy.model_management`` (the one
     ComfyUI module it imports).  Returns the package's modules or None when it was not installed."""
     pkg = os.path.join(REF_DIR, "comfyui_propainter_nodes")
     if not os.path.exists(os.path.join(pkg, "propainter_inference.py")):
@@ -185,7 +186,7 @@ def reference_pass(ref, models, image, mask, device, fp16):
 
 
 def oracle_pass(n_frames):
-    """CPU oracle port on the first `n_frames` frames of the clip (only used when baseline/_ref is absent)."""
+    """CPU oracle port on the first `n_frames` frames of the clip (only used when oracle/_ref is absent)."""
     from comfyui_propainter_nodes_b200.utils import image_utils as IU
     from oracle import propainter_oracle as O
     image, mask = synthetic_inputs()
@@ -222,7 +223,7 @@ def run_reference(args, rank):
     if args.warmup > 0:
         cpu_sample(3)            # thread pools, allocator and first-touch of the weights
     v, dt, kind, cores = cpu_sample(n)
-    what = "the unmodified reference (baseline/_ref), fp32, PyTorch CPU" if kind == "reference" else "CPU oracle port of the reference, fp32"
+    what = "the unmodified reference (oracle/_ref), fp32, PyTorch CPU" if kind == "reference" else "CPU oracle port of the reference, fp32"
     sample = (f"ONE pass over the first {n} frames of the 80-frame 640x360 clip (raft_iter=20, all other parameters of the "
               f"workload), {what}, {cores} threads, {dt:.1f} s")
     line = {
@@ -233,7 +234,7 @@ def run_reference(args, rank):
         "e2e": {"value": v, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "note": "timed once (a 16-frame pass is tens of seconds); --steps/--warmup of the command line are not repeated",
     }
-    # second stated baseline: the reference's own PyTorch-CUDA fp16 path on this B200 at the full workload
+    # second stated baseline: the reference's own PyTorch-CUDA fp16 path on this GPU at the full workload
     if kind == "reference" and torch.cuda.is_available() and not args.no_ref_cuda:
         try:
             ref = load_reference()
@@ -253,8 +254,16 @@ def run_reference(args, rank):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# B200 arm
+# CUDA-engine arm
 # ------------------------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, frames):
+    """The composited uint8 frames [T, H, W, 3] of the last timed step as float32 .npy; every 4th frame keeps the file
+    under 64 MB (20 of the 80 frames at 640x360: 55 MB)."""
+    os.makedirs(out_dir, exist_ok=True)
+    a = frames.cpu().numpy() if torch.is_tensor(frames) else np.asarray(frames)
+    np.save(os.path.join(out_dir, "composited_frames_every4th.npy"), np.ascontiguousarray(a[::4]).astype(np.float32))
+
+
 def run_b200(args, rank, world):
     import torch.distributed as dist
     from comfyui_propainter_nodes_b200 import propainter_inference as PI
@@ -285,7 +294,7 @@ def run_b200(args, rank, world):
 
     image, mask, ft, fm, md, orig_dev, cfg = prepared(T_FRAMES)
     eng.reserve_for_clip(T_FRAMES, HEIGHT, WIDTH)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > L2 (126 MB)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > L2 (50 MB on H100)
 
     def run_clip(ft, fm, md, orig_dev, cfg):
         if strong:
@@ -325,7 +334,7 @@ def run_b200(args, rank, world):
             flush.fill_(1)
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            fn()
+            last_output[0] = fn()
             b.record()
             torch.cuda.synchronize()
             times.append(a.elapsed_time(b))
@@ -335,12 +344,15 @@ def run_b200(args, rank, world):
             dist.all_reduce(total, op=dist.ReduceOp.MAX)
         return float(total.item()) / steps
 
+    last_output = [None]
     for _ in range(args.warmup):
         step()
     sampler = ClockSampler(local)
     sampler.start()
     l0 = eng.launch_count
     ms_per_step = timed(step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_output[0])
     launches = (eng.launch_count - l0) // max(args.steps, 1)
     clips = 1 if (strong or world == 1) else world
     value = clips * T_FRAMES / (ms_per_step / 1000.0)
@@ -417,11 +429,11 @@ def run_b200(args, rank, world):
 
         FL = ("flops are ALGORITHMIC: 2 x output pixels x Cout x kh x kw x Cin/groups of the reference layer "
               "(no padded channels, no block-diagonal zeros)")
-        # the dominant kernel of the step: the TMA halo-tile tcgen05 convolution (every stride-1 conv and every linear)
-        roof = conv_class("conv:halo:", "conv_halo_kernel (TMA halo-tile tcgen05 convolution: every stride-1 conv / linear launch of the step); " + FL)
+        # the dominant kernel of the step: the TMA halo-tile wgmma convolution (every stride-1 conv and every linear)
+        roof = conv_class("conv:halo:", "conv_halo_kernel (TMA halo-tile wgmma convolution: every stride-1 conv / linear launch of the step); " + FL)
         roof["traffic"] = traffic.get("conv_bytes_per_launch")
         roof["traffic_note"] = traffic.get("note")
-        extra.append(conv_class("conv:", "ALL tcgen05 convolution launches (conv_halo_kernel + conv_igemm_kernel + conv_prog_kernel); " + FL))
+        extra.append(conv_class("conv:", "ALL wgmma convolution launches (conv_halo_kernel + conv_igemm_kernel + conv_prog_kernel); " + FL))
         extra.append(conv_class("conv:igemm:", "conv_igemm_kernel (cp.async implicit GEMM: stride-2 / 7x7 / replicate-pad layers, all-pairs correlation)"))
         extra.append(conv_class("conv:prog:", "conv_prog_kernel (multi-layer program: one flow-completion propagation step = 8 dependent layers per launch, "
                                               "latency-bound by construction)"))
@@ -435,7 +447,7 @@ def run_b200(args, rank, world):
         if "attention" in prof:
             v = prof["attention"]
             tf = v["flops"] / (v["ms"] / 1e3) / 1e12 if v["ms"] > 0 else 0.0
-            extra.append({"kernel": "window_attention_tc (tcgen05, masked windows) + window_attention (unmasked windows)", "bound": "tensor",
+            extra.append({"kernel": "window_attention_tc (wgmma, masked windows) + window_attention (unmasked windows)", "bound": "tensor",
                           "achieved": tf, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": tf / pk["tensor"],
                           "flops": "4 x queries x keys x 128 per head of the windows that are actually masked / unmasked in this clip",
                           "ms": v["ms"], "launches": v["count"]})
@@ -449,7 +461,7 @@ def run_b200(args, rank, world):
     if rank == 0 and world == 1 and not args.no_cpu:
         v, dt, kind, cores = cpu_sample(4)
         cpu = {"value": v, "unit": "frames/s", "cores": cores, "kind": kind,
-               "sample": f"first 4 frames of the same clip and parameters ({'unmodified reference from baseline/_ref' if kind == 'reference' else 'CPU oracle port'}, fp32, {dt:.1f} s)"}
+               "sample": f"first 4 frames of the same clip and parameters ({'unmodified reference from oracle/_ref' if kind == 'reference' else 'CPU oracle port'}, fp32, {dt:.1f} s)"}
     if rank == 0:
         if strong:
             par = (f"ONE subvideo sharded over {world} GPUs: RAFT pairs, flow-completion encoder/decoder frames and direction passes, "
@@ -463,7 +475,7 @@ def run_b200(args, rank, world):
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
             "scaling": "weak" if (world > 1 and not strong) else "strong",
             "vs_baseline": None, "dtype": "f16", "data": "synthetic",
-            "config": {"workload": WORKLOAD + (", ONE clip shared by all GPUs" if strong else ", 1 clip per B200"),
+            "config": {"workload": WORKLOAD + (", ONE clip shared by all GPUs" if strong else ", 1 clip per GPU"),
                        "frames_per_gpu": T_FRAMES / world if strong else T_FRAMES, "l2": "flushed between steps (256 MiB write)",
                        "weights": "seeded synthetic checkpoints", "parallelism": par,
                        "e2e_inputs": "pageable host tensors (what ComfyUI hands a node); result in a pinned block of torch's caching host allocator",
@@ -491,6 +503,8 @@ def main():
     ap.add_argument("--no-config2", action="store_true", help="skip the 240-frame config[2] leg")
     ap.add_argument("--no-ref-cuda", action="store_true", help="reference arm: skip the reference's PyTorch-CUDA leg")
     ap.add_argument("--profile-out", default=None, help="write the full per-kernel table (JSON) here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float32, seeded inputs)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))

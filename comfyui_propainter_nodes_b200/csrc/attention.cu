@@ -9,7 +9,7 @@
 // scale 1/sqrt(128), softmax, PV.  fp16 operands, fp32 accumulation and softmax statistics.
 //
 // This file: warp-level mma.sync.m16n8k16 kernel used for the UNMASKED windows (45 queries x 45 keys per frame,
-// a shape far below a tcgen05 tile); masked windows -- where the FLOPs are -- run on the tcgen05/TMEM kernel
+// a shape far below a wgmma tile); masked windows -- where the FLOPs are -- run on the wgmma kernel
 // in attention_tc.cu.  CTA = 4 warps = 64 query rows, key tiles of 64.
 #include "attention.cuh"
 #include "kernels.cuh"
@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(NT) window_attention(const AttnParams p) {
   const int frame_base = p.sw_frame_off[sw];
   const int n_tind = (t - p.parity + 1) / 2;
   const bool masked = p.win_flags[sw * p.n_win + win] != 0;
-  if (masked && p.only_unmasked) return;     // masked windows run on the tcgen05 kernel (attention_tc.cu)
+  if (masked && p.only_unmasked) return;     // masked windows run on the wgmma kernel (attention_tc.cu)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   int nq, nk, q_frame0;
@@ -234,7 +234,7 @@ int pp_k_attention(const __half* q, const __half* k, const __half* v, int qkv_cs
   p.scale_log2 = 1.4426950408889634f / sqrtf((float)D);
   p.only_unmasked = 1;
   p.key_tab = key_tab; p.key_tab_stride = key_tab_stride;
-  PP_TRY(pp_launch_attention_tc(p, n_sliding, t_max, st));   // masked windows: tcgen05 / TMEM
+  PP_TRY(pp_launch_attention_tc(p, n_sliding, t_max, st));   // masked windows: wgmma
   dim3 grid(t_max, p.n_win * 4, n_sliding);                  // unmasked windows: one 45x45 problem per frame
   const size_t smem = (size_t)(BQ + 4 * BKEY) * 256;
   static bool attr_set = false;

@@ -1,5 +1,5 @@
 // Shared parameter block of the two window-attention kernels (attention.cu: mma.sync, unmasked windows;
-// attention_tc.cu: tcgen05/TMEM, masked windows).
+// attention_tc.cu: wgmma, masked windows).
 #pragma once
 #include "pp_common.cuh"
 

@@ -1,24 +1,21 @@
-// Masked-window attention on tcgen05 tensor cores (SparseWindowAttention, sparse_transformer.py:327-357).
+// Masked-window attention on Hopper tensor cores (SparseWindowAttention, sparse_transformer.py:327-357).
 //
-// One CTA (256 threads, two per SM) per (128-query tile, 5x9 window, head, sliding window).  Per 64-key tile:
-//   S = Q K^T       tcgen05.mma  M=128 (queries) N=64 (keys) K=128 (d)    -> TMEM columns [0,64)
-//   softmax         threads r and r+128 own query row r (= TMEM lane r), 32 key columns each: tcgen05.ld, online
-//                   max/sum in registers (one shared-memory exchange of the row max per tile, no shuffles),
+// One CTA (256 threads = two warpgroups, two CTAs per SM) per (128-query tile, 5x9 window, head, sliding window);
+// warpgroup w owns query rows 64w..64w+63.  Per 64-key tile:
+//   S = Q K^T       wgmma m64n64k16 x8 (K = 128 = d)                    -> registers
+//   softmax         in registers: a query row lives on the 4 threads of a quad (row max / sum by two shuffles),
 //                   P (fp16) written to shared memory as the next A operand
-//   O += P V        tcgen05.mma  M=128 N=128 (d) K=64 (keys), V as the MN-major B operand  -> TMEM [128,256)
-// O stays in TMEM for the whole key loop.  The running max is only raised when it grew by more than 8 (log2
-// units), in which case the O rows are rescaled in TMEM (tcgen05.ld/st); softmax is invariant to that shift, so
-// the result is exact while P stays within fp16 range (<= 2^8).
+//   O += P V        wgmma m64n128k16 x4 (K = 64 keys), V as the MN-major B operand  -> registers
+// The running max is only raised when it grew by more than 8 (log2 units), in which case the O rows are rescaled;
+// softmax is invariant to that shift, so the result is exact while P stays within fp16 range (<= 2^8).
 // Keys are gathered by index (own 45 + ring 148 + pooled tokens of every 2nd frame) with 16-byte cp.async into
 // 128B-swizzled panels -- the window/rolled/pooled K,V tensors of the reference are never materialised.
 #include "attention.cuh"
+#include "wgmma_ops.cuh"
 
 namespace {
 
 constexpr int D = 128, BQ = 128, BKEY = 64, NT = 256, WIN_TOK = 45, RING = 193;
-constexpr int CPT = BKEY / 2;
-constexpr int TMEM_COLS = 256;                 // S: BKEY columns at 0, O: 128 columns at O_COL
-constexpr int O_COL = 128;                   // key columns per thread (two threads per query row)
 constexpr uint32_t QPANEL = BQ * 128;           // bytes of a [128 rows][64 halves] panel (Q, P)
 constexpr uint32_t KPANEL = BKEY * 128;         // bytes of a [BKEY rows][64 halves] panel (K, V)
 constexpr uint32_t QTILE = 2 * QPANEL;          // Q: [128][128 d]
@@ -54,11 +51,6 @@ __global__ void __launch_bounds__(NT, 2) window_attention_tc(const PPAttnParams 
   using namespace ppx;
   extern __shared__ __align__(1024) uint8_t smem[];   // 128B-swizzled tiles need 1024-byte alignment
   const uint32_t sbase = smem_u32(smem);
-  uint64_t* mbar_s = reinterpret_cast<uint64_t*>(smem + SM_END);
-  uint64_t* mbar_o = mbar_s + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(mbar_o + 1);
-  __half* xmax = reinterpret_cast<__half*>(smem + SM_END + 64);   // [2][128] per-tile row-max exchange
-  float* xsum = reinterpret_cast<float*>(smem + SM_Q);            // [2][128] row-sum exchange (Q tile is dead by then)
 
   const int win = blockIdx.y >> 2, head = blockIdx.y & 3, sw = blockIdx.z;
   if (p.win_flags[sw * p.n_win + win] == 0) return;        // unmasked windows: mma.sync kernel
@@ -71,19 +63,9 @@ __global__ void __launch_bounds__(NT, 2) window_attention_tc(const PPAttnParams 
   const int kpf = RING + p.n_pool;
   const int nk = n_tind * kpf;
   const int ntiles = (nk + BKEY - 1) / BKEY;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int* ring = p.ring_idx + win * RING;
   const long long ntok = (long long)p.nh * p.nw;
-
-  if (tid == 0) {
-    mbar_init(mbar_s, 1);
-    mbar_init(mbar_o, 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
 
   // ---- Q tile (rows beyond nq are clamped to a valid query; never stored)
   for (int i = tid; i < BQ * 16; i += NT) {
@@ -124,152 +106,109 @@ __global__ void __launch_bounds__(NT, 2) window_attention_tc(const PPAttnParams 
   };
   load_kv(0, 0);   // one group: Q + first K/V tile
 
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int row = tid & 127, half = tid >> 7;                             // query row, which 64 key/d columns
-  const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);   // this thread's TMEM lane (= query row)
-  const uint32_t idesc_s = umma_idesc_f16(128, BKEY);
-  const uint32_t idesc_o = umma_idesc_f16_bmn(128, 128);
-
-  float m_used = 0.f, m_run = -1e30f, row_sum = 0.f;
+  // fragment coordinates (pp_common.cuh): this thread holds rows rw and rw + 8 of its warpgroup's 64, and per 8-column
+  // group the two columns 2 * quad .. +1
+  const int wg = tid >> 7, lane = tid & 31;
+  const int rw = 16 * ((tid >> 5) & 3) + (lane >> 2), quad = lane & 3;
+  const uint32_t q_rows = (uint32_t)wg * 64 * 128;   // byte offset of this warpgroup's rows in a [128][64] panel
+  float o[64];
+  float m_used[2] = {0.f, 0.f}, m_run[2] = {-1e30f, -1e30f}, row_sum[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
   for (int j = 0; j < ntiles; ++j) {
     const int stage = j & 1;
     cp_async_wait<0>();
     fence_proxy_async();
-    __syncthreads();
-    if (warp == 0 && elect_one()) {   // S = Q K^T (one elected lane: ptxas emits each UTCHMMA once)
-      tc_fence_after();
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) {
-        const uint32_t sub = (uint32_t)(ks & 3) * 32;
-        umma_f16(tmem_base, umma_desc_sw128_kmajor(sbase + SM_Q + (uint32_t)(ks >> 2) * QPANEL + sub),
-                 umma_desc_sw128_kmajor(sbase + SM_K + stage * KTILE + (uint32_t)(ks >> 2) * KPANEL + sub), idesc_s,
-                 ks != 0 ? 1u : 0u);
-      }
-      umma_commit(mbar_s);
-    }
-    // previous P.V must be done before its K/V stage and the P buffer are overwritten
-    if (j > 0) { mbar_wait(mbar_o, (uint32_t)(j - 1) & 1u); tc_fence_after(); }
+    __syncthreads();   // K/V tile j has landed; both warpgroups are done with tile j-1 (its stage is free again)
     if (j + 1 < ntiles) load_kv(j + 1, stage ^ 1);
-    mbar_wait(mbar_s, (uint32_t)j & 1u);
-    tc_fence_after();
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t sub = (uint32_t)(ks & 3) * 32;
+      wgmma_f16<BKEY>(s, gmma_desc_sw128_kmajor(sbase + SM_Q + (uint32_t)(ks >> 2) * QPANEL + q_rows + sub),
+                      gmma_desc_sw128_kmajor(sbase + SM_K + stage * KTILE + (uint32_t)(ks >> 2) * KPANEL + sub), ks != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
 
-    // ---- this thread's CPT columns of its S row
-    float s[CPT];
+    const int kvalid = min(BKEY, nk - j * BKEY);
+    float mx[2] = {-1e30f, -1e30f};
 #pragma unroll
-    for (int c = 0; c < CPT / 16; ++c) {
-      uint32_t raw[16];
-      tmem_ld16(lane_addr + half * CPT + c * 16, raw);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) s[c * 16 + i] = __uint_as_float(raw[i]);
+    for (int i = 0; i < 32; ++i) {
+      if (8 * (i >> 2) + 2 * quad + (i & 1) >= kvalid) s[i] = -1e30f;
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
     }
-    tmem_ld_wait();
-    const int kvalid = min(BKEY, nk - j * BKEY) - half * CPT;   // valid columns among this thread's
-    if (kvalid < CPT) {
+    float f[2];
 #pragma unroll
-      for (int i = 0; i < CPT; ++i) if (i >= kvalid) s[i] = -1e30f;
-    }
-    float mx[4] = {-1e30f, -1e30f, -1e30f, -1e30f};
-#pragma unroll
-    for (int i = 0; i < CPT; i += 4) {
-      mx[0] = fmaxf(mx[0], s[i]); mx[1] = fmaxf(mx[1], s[i + 1]); mx[2] = fmaxf(mx[2], s[i + 2]); mx[3] = fmaxf(mx[3], s[i + 3]);
-    }
-    // both threads of a row read the same two (fp16-rounded) values, so they agree on the reference max; any
-    // reference works for softmax as long as numerator and denominator share it
-    xmax[half * 128 + row] = __float2half_rn(fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])) * p.scale_log2, -60000.f));
-    __syncthreads();
-    const float m_tile = fmaxf(__half2float(xmax[row]), __half2float(xmax[128 + row]));
-    const float m_new = fmaxf(m_run, m_tile);
-    int need = 0;
-    if (j == 0) m_used = m_new;
-    else need = m_new > m_used + 8.f;
-    m_run = m_new;
-    if (__syncthreads_or(need)) {
-      // rare: raise the reference max of the rows that need it and rescale their O rows in TMEM
-      const float f = need ? exp2f(m_used - m_new) : 1.f;
-      if (need) { m_used = m_new; row_sum *= f; }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t raw[16];
-        tmem_ld16(lane_addr + O_COL + half * 64 + c * 16, raw);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) raw[i] = __float_as_uint(__uint_as_float(raw[i]) * f);
-        tmem_st16(lane_addr + O_COL + half * 64 + c * 16, raw);
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      // the reference max is kept in fp16 precision; any reference works for softmax as long as numerator and
+      // denominator share it
+      const float m_tile = __half2float(__float2half_rn(fmaxf(mx[h] * p.scale_log2, -60000.f)));
+      const float m_new = fmaxf(m_run[h], m_tile);
+      f[h] = 1.f;
+      if (j == 0) m_used[h] = m_new;
+      else if (m_new > m_used[h] + 8.f) {   // rare: raise the reference max and rescale the row
+        f[h] = exp2f(m_used[h] - m_new);
+        m_used[h] = m_new;
+        row_sum[h] *= f[h];
       }
-      tmem_st_wait();
+      m_run[h] = m_new;
     }
-    // ---- P = exp2(s*scale - m_used) -> shared memory (A operand of P.V): this thread's 16-byte chunks
-    float ps[4] = {0.f, 0.f, 0.f, 0.f};
+    if (f[0] != 1.f || f[1] != 1.f) {
 #pragma unroll
-    for (int ch = 0; ch < CPT / 8; ++ch) {
-      __align__(16) __half2 h[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float a = exp2f(fmaf(s[ch * 8 + 2 * e], p.scale_log2, -m_used));
-        const float b = exp2f(fmaf(s[ch * 8 + 2 * e + 1], p.scale_log2, -m_used));
-        ps[e] += a + b;
-        h[e] = __floats2half2_rn(a, b);
-      }
-      *reinterpret_cast<uint4*>(smem + SM_P + tile_off(QPANEL, row, half * (CPT / 8) + ch)) = *reinterpret_cast<uint4*>(h);
+      for (int i = 0; i < 64; ++i) o[i] *= f[(i >> 1) & 1];
     }
-    row_sum += (ps[0] + ps[1]) + (ps[2] + ps[3]);
+    // ---- P = exp2(s*scale - m_used) -> shared memory (A operand of P.V)
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float a = exp2f(fmaf(s[i], p.scale_log2, -m_used[h]));
+      const float b = exp2f(fmaf(s[i + 1], p.scale_log2, -m_used[h]));
+      row_sum[h] += a + b;
+      const int row = wg * 64 + rw + 8 * h;
+      *reinterpret_cast<__half2*>(smem + SM_P + tile_off(QPANEL, row, i >> 2) + 4 * quad) = __floats2half2_rn(a, b);
+    }
     fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0 && elect_one()) {   // O += P V
-      tc_fence_after();
+    named_bar(1 + wg, 128);   // this warpgroup's P rows are complete
+    wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < BKEY / 16; ++ks) {
-        const uint64_t adesc = umma_desc_sw128_kmajor(sbase + SM_P + (uint32_t)(ks >> 2) * QPANEL + (uint32_t)(ks & 3) * 32);
-        const uint64_t bdesc = umma_desc_sw128_mnmajor(sbase + SM_V + stage * KTILE + (uint32_t)ks * 2048, KPANEL);
-        umma_f16(tmem_base + O_COL, adesc, bdesc, idesc_o, (j | ks) != 0 ? 1u : 0u);
-      }
-      umma_commit(mbar_o);
+    for (int ks = 0; ks < BKEY / 16; ++ks) {
+      const uint64_t adesc = gmma_desc_sw128_kmajor(sbase + SM_P + q_rows + (uint32_t)ks * 32);
+      const uint64_t bdesc = gmma_desc_sw128_mnmajor(sbase + SM_V + stage * KTILE + (uint32_t)ks * 2048, KPANEL);
+      wgmma_f16<D, 1>(o, adesc, bdesc, 1u);
     }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(o);
   }
 
   // ---- epilogue: O / row_sum -> global (unpadded grid; padding queries are dropped)
-  mbar_wait(mbar_o, (uint32_t)(ntiles - 1) & 1u);
-  tc_fence_after();
-  xsum[half * 128 + row] = row_sum;
-  __syncthreads();
-  const float inv = 1.f / (xsum[row] + xsum[128 + row]);
-  const int qi = q0 + row;
-  bool store = qi < nq;
-  __half* dst = nullptr;
-  if (store) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    row_sum[h] += __shfl_xor_sync(0xffffffffu, row_sum[h], 1);
+    row_sum[h] += __shfl_xor_sync(0xffffffffu, row_sum[h], 2);
+    const float inv = 1.f / row_sum[h];
+    const int qi = q0 + wg * 64 + rw + 8 * h;
+    if (qi >= nq) continue;
     const int fr = frame_base + qi / WIN_TOK, pos = qi % WIN_TOK;
     const int tok = ring[pos];
     const int ty = tok / p.nw, tx = tok - ty * p.nw;
-    store = ty < p.gh && tx < p.gw;
-    dst = p.out + (((long long)fr * p.gh + ty) * p.gw + tx) * p.out_cs + head * D + half * 64;
-  }
+    if (ty >= p.gh || tx >= p.gw) continue;
+    __half* dst = p.out + (((long long)fr * p.gh + ty) * p.gw + tx) * p.out_cs + head * D + 2 * quad;
 #pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    uint32_t raw[16];
-    tmem_ld16(lane_addr + O_COL + half * 64 + c * 16, raw);
-    tmem_ld_wait();
-    if (store) {
-      __align__(16) __half2 h[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        h[i] = __floats2half2_rn(__uint_as_float(raw[2 * i]) * inv, __uint_as_float(raw[2 * i + 1]) * inv);
-      reinterpret_cast<uint4*>(dst + c * 16)[0] = reinterpret_cast<uint4*>(h)[0];
-      reinterpret_cast<uint4*>(dst + c * 16)[1] = reinterpret_cast<uint4*>(h)[1];
-    }
+    for (int g = 0; g < D / 8; ++g)
+      *reinterpret_cast<__half2*>(dst + 8 * g) = __floats2half2_rn(o[4 * g + 2 * h] * inv, o[4 * g + 2 * h + 1] * inv);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 }  // namespace
 
 int pp_launch_attention_tc(const PPAttnParams& p, int n_sliding, int t_max, cudaStream_t st) {
-  const size_t smem = SM_END + 64 + 2 * 128 * sizeof(__half);   // 115,264 B: two CTAs per SM
+  const size_t smem = SM_END;   // 112 KiB: two CTAs per SM
   static bool attr_set = false;
   if (!attr_set) {
     PP_CUDA_CHECK(cudaFuncSetAttribute(window_attention_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

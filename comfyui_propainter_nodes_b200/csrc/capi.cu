@@ -51,7 +51,7 @@ struct ArenaGuard {
 
 extern "C" {
 
-const char* pp_version(void) { return "propainter_b200 1 sm_100a"; }
+const char* pp_version(void) { return "propainter_b200 1 sm_90a"; }
 
 int pp_create(int device, void* workspace, size_t workspace_bytes, pp_handle* out) {
   PP_REQUIRE(out != nullptr, "pp_create: out is null");
@@ -60,7 +60,7 @@ int pp_create(int device, void* workspace, size_t workspace_bytes, pp_handle* ou
   PP_CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   PP_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  PP_REQUIRE(prop.major == 10, "pp_create: this library is built for sm_100a (Blackwell B200); device %d is sm_%d%d",
+  PP_REQUIRE(prop.major == 9 && prop.minor == 0, "pp_create: this library is built for sm_90a (Hopper H100); device %d is sm_%d%d",
              device, prop.major, prop.minor);
   PPEngine* e = new PPEngine();
   e->device = device;

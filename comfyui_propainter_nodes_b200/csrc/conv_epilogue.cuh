@@ -1,7 +1,8 @@
-// Epilogue shared by the tcgen05 conv kernels: 16 consecutive output channels of one output pixel
+// Epilogue shared by the wgmma conv kernels: 16 consecutive output channels of one output pixel
 // (accumulators already in registers) -> bias / activation / residual / GRU gate fusions -> global memory.
 #pragma once
 #include "conv_igemm.cuh"
+#include "wgmma_ops.cuh"
 
 namespace ppconv {
 
@@ -28,19 +29,6 @@ __device__ __forceinline__ void act16(float (&v)[16], int act, float slope) {
   }
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): 16 fp16 channels of one pixel in ONE request, so a warp's
-// store touches each of its 32 rows' sectors once instead of twice.
-__device__ __forceinline__ void ldg256(const void* p, uint4& a, uint4& b) {
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-               : "l"(p));
-}
-__device__ __forceinline__ void stg256(void* p, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w),
-               "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
-}
-
 // 16 consecutive fp16 values <-> registers.  `vec` (uniform per launch, checked on the host) says that full
 // runs are 16-byte aligned, so they move as 2 x 16-byte accesses; partial runs take the scalar tail.
 __device__ __forceinline__ void load16(const __half* src, int nvalid, bool vec, float (&r)[16]) {
@@ -58,15 +46,11 @@ __device__ __forceinline__ void load16(const __half* src, int nvalid, bool vec, 
     for (int i = 0; i < 16; ++i) r[i] = i < nvalid ? __half2float(src[i]) : 0.f;
   }
 }
-__device__ __forceinline__ void store16(__half* dst, int nvalid, bool vec, const float (&v)[16], bool v32 = false) {
+__device__ __forceinline__ void store16(__half* dst, int nvalid, bool vec, const float (&v)[16]) {
   if (vec && nvalid == 16) {
     __align__(16) __half2 h[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    if (v32) {
-      stg256(dst, reinterpret_cast<uint4*>(h)[0], reinterpret_cast<uint4*>(h)[1]);
-      return;
-    }
     reinterpret_cast<uint4*>(dst)[0] = reinterpret_cast<uint4*>(h)[0];
     reinterpret_cast<uint4*>(dst)[1] = reinterpret_cast<uint4*>(h)[1];
   } else {
@@ -86,8 +70,8 @@ __device__ __forceinline__ void unpack16(const uint4& a, const uint4& b, float (
   }
 }
 
-// Epilogue operands that do not depend on the accumulator (residual / GRU h and z), fetched while the TMEM read of
-// the same 16 columns is still in flight so the two latencies overlap instead of adding up.
+// Epilogue operands that do not depend on the accumulator (residual / GRU h and z), fetched before the accumulator of the same
+// 16 columns is read back so the two latencies overlap instead of adding up.
 struct EpiAux {
   uint4 a0[2], a1[2];
   bool have;
@@ -109,11 +93,6 @@ __device__ __forceinline__ void conv_epilogue_prefetch16(const PPConvParams& p, 
   }
   if (s0 == nullptr) return;
   x.have = true;
-  if (p.vec32_ok) {
-    ldg256(s0, x.a0[0], x.a0[1]);
-    if (s1 != nullptr) ldg256(s1, x.a1[0], x.a1[1]);
-    return;
-  }
   x.a0[0] = reinterpret_cast<const uint4*>(s0)[0];
   x.a0[1] = reinterpret_cast<const uint4*>(s0)[1];
   if (s1 != nullptr) {
@@ -122,7 +101,7 @@ __device__ __forceinline__ void conv_epilogue_prefetch16(const PPConvParams& p, 
   }
 }
 
-// `raw`: 16 fp32 accumulators (TMEM columns ng0-n0 .. +15) of output pixel `mrow` (flattened N*OH*OW index),
+// `raw`: 16 fp32 accumulators (tile columns ng0-n0 .. +15) of output pixel `mrow` (flattened N*OH*OW index),
 // group g, first channel ng0 (within the group; ng0 < Cout_g).  `epi`/`vec` are launch-uniform.
 // sm0 / sm1 (STD epilogue, fp16 output only): when non-null the 16 results go to these two 16-byte shared-memory slots
 // (a staging tile that a TMA store writes out) instead of global memory.
@@ -130,7 +109,6 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
                                                 int ng0, int epi, bool vec, const EpiAux* pre = nullptr,
                                                 uint4* sm0 = nullptr, uint4* sm1 = nullptr) {
     const int nvalid = min(16, p.Cout_g - ng0);
-    const bool v32 = p.vec32_ok != 0;
     float v[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(raw[i]);
@@ -181,13 +159,13 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
         *sm0 = reinterpret_cast<uint4*>(h)[0];
         *sm1 = reinterpret_cast<uint4*>(h)[1];
       } else {
-        store16(reinterpret_cast<__half*>(p.out) + o, nvalid, vec, v, v32);
+        store16(reinterpret_cast<__half*>(p.out) + o, nvalid, vec, v);
       }
     } else if (epi == PP_EPI_GRU_ZR) {
       const int half_c = p.Cout_g >> 1;
       act16_t<PP_ACT_SIGMOID>(v, 0.f);
       if (ng0 < half_c) {
-        store16(reinterpret_cast<__half*>(p.out) + mrow * p.out_cstride + p.out_coff + ng0, nvalid, vec, v, v32);
+        store16(reinterpret_cast<__half*>(p.out) + mrow * p.out_cstride + p.out_coff + ng0, nvalid, vec, v);
       } else {
         const int c = ng0 - half_c;
         float h[16];
@@ -195,7 +173,7 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
         else load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + c, nvalid, vec, h);
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] *= h[i];
-        store16(p.out2 + mrow * p.out2_cstride + p.out2_coff + c, nvalid, vec, v, v32);
+        store16(p.out2 + mrow * p.out2_cstride + p.out2_coff + c, nvalid, vec, v);
       }
     } else {  // PP_EPI_GRU_H
       float h[16], z[16];
@@ -209,8 +187,89 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
       act16_t<PP_ACT_TANH>(v, 0.f);
 #pragma unroll
       for (int i = 0; i < 16; ++i) v[i] = (1.f - z[i]) * h[i] + z[i] * v[i];
-      store16(reinterpret_cast<__half*>(p.out) + mrow * p.out_cstride + p.out_coff + ng0, nvalid, vec, v, v32);
+      store16(reinterpret_cast<__half*>(p.out) + mrow * p.out_cstride + p.out_coff + ng0, nvalid, vec, v);
     }
+}
+
+// ---- accumulator hand-off for the wgmma kernels
+// A warpgroup's m64 x N accumulator is spread over its 128 threads in the wgmma fragment layout (pp_common.cuh); the
+// epilogue wants 16 consecutive channels of one pixel per thread.  Per 32-column chunk the warpgroup writes its
+// fragments into a [64][STG_LD] fp32 staging tile, meets on a named barrier, and thread t takes row t / 2, columns
+// 16 * (t % 2) .. +15 of the chunk.
+constexpr int STG_LD = 40;                  // floats per row: the float2 writes of a half-warp hit 32 distinct banks
+constexpr int STG_BYTES = 64 * STG_LD * 4;  // per warpgroup
+
+// `emit(src, r, c)`: 16 fp32 values at `src` are columns c .. c+15 of row r (0..63) of the accumulator.  The chunk loop
+// is a runtime loop (one inlined copy of the epilogue); only the register -> staging copy is unrolled per chunk.
+template <int N, class Emit>
+__device__ __forceinline__ void drain_acc(const float (&acc)[N / 2], float* stg, int t128, int bar_id, Emit&& emit) {
+  const int wrow = 16 * (t128 >> 5) + ((t128 & 31) >> 2), wcol = 2 * (t128 & 3);
+#pragma unroll 1
+  for (int c0 = 0; c0 < N; c0 += 32) {
+#pragma unroll
+    for (int cc = 0; cc < N; cc += 32) {
+      if (cc == c0) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          if (cc + 8 * j < N) {
+            const int i = (cc / 8 + j) * 4;
+            *reinterpret_cast<float2*>(stg + wrow * STG_LD + 8 * j + wcol) = make_float2(acc[i], acc[i + 1]);
+            *reinterpret_cast<float2*>(stg + (wrow + 8) * STG_LD + 8 * j + wcol) = make_float2(acc[i + 2], acc[i + 3]);
+          }
+        }
+      }
+    }
+    ppx::named_bar(bar_id, 128);
+    const int c = c0 + 16 * (t128 & 1);
+    if (c < N) emit(stg + (t128 >> 1) * STG_LD + 16 * (t128 & 1), t128 >> 1, c);
+    ppx::named_bar(bar_id, 128);
+  }
+}
+
+// conv_epilogue16 on 16 staged accumulators
+__device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const float* src, long long mrow, int g, int ng0,
+                                                    uint4* sm0, uint4* sm1) {
+  uint32_t raw[16];
+#pragma unroll
+  for (int i = 0; i < 16; i += 4) {
+    const float4 v = *reinterpret_cast<const float4*>(src + i);
+    raw[i] = __float_as_uint(v.x); raw[i + 1] = __float_as_uint(v.y);
+    raw[i + 2] = __float_as_uint(v.z); raw[i + 3] = __float_as_uint(v.w);
+  }
+  conv_epilogue16(p, raw, mrow, g, ng0, p.epi, p.vec_ok != 0, nullptr, sm0, sm1);
+}
+
+// f(IntC<BN>{}) for the runtime tile width bn (a multiple of 16, at most MAX_N)
+template <int V>
+struct IntC { static constexpr int value = V; };
+template <int MAX_N, class F>
+__device__ __forceinline__ void with_tile_width(int bn, F&& f) {
+  switch (bn) {
+    case 16: f(IntC<16>{}); break;
+    case 32: f(IntC<32>{}); break;
+    case 48: f(IntC<48>{}); break;
+    case 64: f(IntC<64>{}); break;
+    case 80: f(IntC<80>{}); break;
+    case 96: f(IntC<96>{}); break;
+    case 112: f(IntC<112>{}); break;
+    case 128: f(IntC<128>{}); break;
+    default:
+      if constexpr (MAX_N > 128) {
+        switch (bn) {
+          case 144: f(IntC<144>{}); break;
+          case 160: f(IntC<160>{}); break;
+          case 176: f(IntC<176>{}); break;
+          case 192: f(IntC<192>{}); break;
+          case 208: f(IntC<208>{}); break;
+          case 224: f(IntC<224>{}); break;
+          case 240: f(IntC<240>{}); break;
+          case 256: f(IntC<256>{}); break;
+          default: __trap();
+        }
+      } else {
+        __trap();
+      }
+  }
 }
 
 }  // namespace ppconv

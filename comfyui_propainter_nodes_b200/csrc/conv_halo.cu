@@ -1,4 +1,4 @@
-// Halo-tile tcgen05 convolution for sm_100a: stride-1 convolutions whose A operand is fed by TMA.
+// Halo-tile wgmma convolution for sm_90a: stride-1 convolutions whose A operand is fed by TMA.
 //
 // The implicit-GEMM kernel (conv_igemm.cu) fetches every input element once per filter tap (9x for a 3x3) with
 // cp.async and streams the weight tile once per 128 output pixels; on the 3x3 / 1x5 / 5x1 layers with <= 256
@@ -7,16 +7,16 @@
 //   * per 64-channel chunk, ONE 4-D TMA box load (cp.async.bulk.tensor, SWIZZLE_128B, out-of-image coordinates
 //     zero-filled = the conv's zero padding) lands the input patch [(16+(kh-1)dh) x (8MT+(kw-1)dw)] pixels x 128 B
 //     in shared memory; the A operand of filter tap (ky,kx) of sub-tile s is a *shifted view* of that patch:
-//     UMMA descriptor start = patch + ((ky*dh)*BW + kx*dw + 8s)*128 B, stride between 8-pixel row groups
+//     wgmma descriptor start = patch + ((ky*dh)*BW + kx*dw + 8s)*128 B, stride between 8-pixel row groups
 //     (SBO) = BW*128 B.  The 128B swizzle is a function of the absolute shared-memory address, so views that are
-//     not 1024-byte aligned are consistent with what TMA wrote (verified on B200: tools/umma_probe.cu).
+//     not 1024-byte aligned are consistent with what TMA wrote.
 //   * the weight tile of (chunk, tap) [BN x 64] is streamed once per tile with cp.async.bulk and feeds both
 //     sub-tiles, so weights move once per 256 output pixels.
 // L2->SM bytes per output pixel drop ~3x on a 3x3 Cin=256 Cout=128 layer and no thread issues per-element loads.
 //
-// Warp roles (352 threads, one persistent CTA per SM): warps 0-7 epilogue (TMEM -> registers -> fused epilogue of
-// conv_epilogue.cuh -> global), warp 8 patch producer (TMA), warp 9 weight producer (bulk copy), warp 10 MMA issuer
-// + TMEM allocation.  Two accumulator sets in TMEM (2 x MT x BN columns) overlap epilogue i with main loop i+1.
+// Warp roles (384 threads, one persistent CTA per SM): warpgroups 0-1 consumers (wgmma into register accumulators,
+// then the fused epilogue of conv_epilogue.cuh -> global), warp 8 patch producer (TMA), warp 9 weight producer (bulk
+// copy).  MT == 1: warpgroup w owns pixel rows 64w..64w+63 of the sub-tile; MT == 2: warpgroup w owns sub-tile w.
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -29,15 +29,16 @@
 
 namespace {
 
-constexpr int NUM_THREADS = 352;
-constexpr int NUM_EPI_THREADS = 256;
-constexpr int WARP_A = 8, WARP_B = 9, WARP_MMA = 10;
+constexpr int NUM_THREADS = 384;   // warpgroup 2: warps 8-9 producers, 10-11 idle (setmaxnreg works per warpgroup)
+constexpr int NUM_EPI_THREADS = 256;   // the two consumer warpgroups
+constexpr int WARP_A = 8, WARP_B = 9;
 // fused x2-upsample variant (UPS): warps 8-11 interpolate the input patch (warp 8 also issues the low-res TMA loads),
-// the weight producer and the MMA issuer move to warps 12 / 13
-constexpr int UPS_THREADS = 448, UPS_INTERP_THREADS = 128;
-constexpr int UPS_WARP_B = 12, UPS_WARP_MMA = 13;
+// the weight producer moves to warp 12
+constexpr int UPS_THREADS = 416, UPS_INTERP_THREADS = 128;
+constexpr int UPS_WARP_B = 12;
 constexpr int MAX_SA = 4, MAX_SB = 8;
-constexpr int SMEM_BUDGET = 208 * 1024;
+// stages; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the barrier block come on top
+constexpr int SMEM_BUDGET = 186 * 1024;
 
 struct HaloParams {
   PPConvParams c;
@@ -48,7 +49,6 @@ struct HaloParams {
   int a_stage_bytes, b_stage_bytes, SA, SB;
   int tps;           // filter taps per weight stage: narrow N tiles pack several taps' [BN x 64] tiles into one stage, so
                      // the MMA issuer waits / commits once per group instead of once per tap (it is issue-bound there)
-  int accw;          // TMEM columns per accumulator
   int chunks;        // Cin / 64
   int flat;          // 1x1 convs: tiles are runs of 128*MT consecutive pixels of the flattened [N*H*W] pixel list
   int n_img;         // images the tile index decomposes over (1 in flat mode)
@@ -92,6 +92,132 @@ __device__ __forceinline__ TileCoord decode_tile(const HaloParams& h, int tile) 
   return t;
 }
 
+// position in a shared-memory ring of stages (consumer side)
+struct Ring {
+  int s;
+  uint32_t ph;
+};
+
+// Consumer side of one tile, run by each of the two consumer warpgroups: the main loop into register accumulators
+// (MB = h.MT m64 blocks of BN columns), then the epilogue of this warpgroup's pixel rows.  A stage is handed back to
+// its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
+template <int BN, int MB>
+__device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, uint8_t* smem, uint8_t* smem_b, int SA, int SB,
+                                          int a_stage_bytes, int b_stage_bytes, uint64_t* a_full, uint64_t* a_empty,
+                                          uint64_t* b_full, uint64_t* b_empty, Ring& ra, Ring& rb, float* stg,
+                                          uint8_t* stg_out, int wg, int t128) {
+  using namespace ppx;
+  const PPConvParams& p = h.c;
+  const int taps = p.kh * p.kw;
+  const TileCoord t = decode_tile(h, tile);
+  const int n0 = t.n_idx * p.BN;
+  const int bnt = min(p.BN, p.Cout_g_pad - n0);   // columns >= bnt of the last N tile read stale weights: never stored
+  const uint32_t sbo = h.flat ? 1024u : (uint32_t)h.BW * 128;
+  const uint32_t step_x = (uint32_t)p.dw * 8;                                 // next tap in the row (16-byte units)
+  const uint32_t step_row = (uint32_t)(p.dh * h.BW - (p.kw - 1) * p.dw) * 8;  // last tap of a row -> next row
+  const uint32_t tap16 = (uint32_t)p.BN * 8;                                  // next tap's weight tile in the stage
+  const int kw = p.kw;
+  uint32_t aoff[MB];
+#pragma unroll
+  for (int b = 0; b < MB; ++b) aoff[b] = MB == 2 ? wg * h.sub_bytes + b * 8 * sbo : wg * 8 * sbo;
+  float acc[MB][BN / 2];
+  uint32_t accum = 0;
+  int pend_a = -1, pend_b = -1;
+  for (int c = 0; c < h.chunks; ++c) {
+    mbar_wait(&a_full[ra.s], ra.ph);
+    uint64_t adesc[MB];
+#pragma unroll
+    for (int b = 0; b < MB; ++b) adesc[b] = gmma_desc_sw128_kmajor(smem_u32(smem + ra.s * a_stage_bytes) + aoff[b], sbo);
+    int kx = 0;
+    for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
+      mbar_wait(&b_full[rb.s], rb.ph);
+      wgmma_fence();
+      uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(smem_b + rb.s * b_stage_bytes));
+      const int tn = min(h.tps, taps - tap0);
+      for (int tt = 0; tt < tn; ++tt) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+          for (int b = 0; b < MB; ++b) wgmma_f16<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (accum | k) != 0 ? 1u : 0u);
+        accum = 1u;
+        bdesc += tap16;
+        const uint32_t step = ++kx == kw ? step_row : step_x;
+        if (kx == kw) kx = 0;
+#pragma unroll
+        for (int b = 0; b < MB; ++b) adesc[b] += step;
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
+      if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+      pend_b = rb.s;
+      pend_a = tap0 + h.tps >= taps ? ra.s : -1;
+      if (++rb.s == SB) { rb.s = 0; rb.ph ^= 1; }
+    }
+    if (++ra.s == SA) { ra.s = 0; ra.ph ^= 1; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int b = 0; b < MB; ++b) wgmma_fence_acc(acc[b]);
+  if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
+  if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+
+  // ---- epilogue.  TMA-store path: staging tile of the sub-tile, its barrier (one warpgroup when MT == 2, both else)
+  const bool skip = (h.debug & 1) != 0;
+  const int bar_id = 2 + (MB == 2 ? wg : 0), bar_n = MB == 2 ? 128 : 256;
+  const bool issuer = t128 == 0 && (MB == 2 || wg == 0);
+  uint8_t* so = h.tstore ? stg_out + (MB == 2 ? wg : 0) * h.out_stage_bytes : nullptr;
+  if (so != nullptr) {
+    if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
+    named_bar(bar_id, bar_n);
+  }
+#pragma unroll
+  for (int b = 0; b < MB; ++b) {
+    const int sub = MB == 2 ? wg : 0, rbase = MB == 2 ? 64 * b : 64 * wg;
+    ppconv::drain_acc<BN>(acc[b], stg, t128, 4 + wg, [&](const float* src, int r64, int cc) {
+      const int r = rbase + r64;   // row of the 128-pixel sub-tile: 16 rows x 8 columns (spatial) or 128 pixels (flat)
+      bool mvalid;
+      long long mrow;
+      if (h.flat) {
+        mrow = ((long long)t.tx * h.MT + sub) * 128 + r;
+        mvalid = mrow < p.M_total;
+      } else {
+        const int oy = t.ty * 16 + (r >> 3), ox = t.tx * (8 * h.MT) + 8 * sub + (r & 7);
+        mvalid = oy < p.OH && ox < p.OW;
+        mrow = ((long long)t.img * p.OH + oy) * p.OW + ox;
+      }
+      if (!mvalid || skip || cc >= bnt || n0 + cc >= p.Cout_g) return;
+      if (so != nullptr) {
+        // 16 columns = two 16-byte units of panel cc/64, row r, 128B swizzle (unit index XOR row & 7)
+        auto slot = [&](int u) {
+          const int unit = ((cc & 63) >> 3) + u;
+          return reinterpret_cast<uint4*>(so + (cc >> 6) * 16384 + r * 128 + ((unit ^ (r & 7)) << 4));
+        };
+        ppconv::epilogue_from_stage(p, src, mrow, t.g, n0 + cc, slot(0), slot(1));
+      } else {
+        ppconv::epilogue_from_stage(p, src, mrow, t.g, n0 + cc, nullptr, nullptr);
+      }
+    });
+  }
+  if (so != nullptr) {
+    fence_proxy_async();                                  // generic-proxy smem writes -> visible to the TMA store
+    named_bar(bar_id, bar_n);
+    if (issuer && !skip) {
+      const int row0 = (int)(((long long)t.tx * h.MT + (MB == 2 ? wg : 0)) * 128);
+      for (int pnl = 0; pnl * 64 < bnt; ++pnl)
+        tma_store_2d(&h.tmap_out, smem_u32(so + pnl * 16384), n0 + pnl * 64, row0);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+  }
+}
+
+// f(IntC<BN>, IntC<MT>) for the layer's runtime tile shape (MT == 2 layers have BN <= 128)
+template <class F>
+__device__ __forceinline__ void with_tile_shape(int mt, int bn, F&& f) {
+  if (mt == 2) ppconv::with_tile_width<128>(bn, [&](auto n) { f(n, ppconv::IntC<2>{}); });
+  else ppconv::with_tile_width<256>(bn, [&](auto n) { f(n, ppconv::IntC<1>{}); });
+}
+
 template <bool UPS>
 __global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_kernel(const __grid_constant__ HaloParams h) {
   using namespace ppx;
@@ -104,130 +230,45 @@ __global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_
   uint64_t* a_empty = a_full + MAX_SA;
   uint64_t* b_full = a_empty + MAX_SA;
   uint64_t* b_empty = b_full + MAX_SB;
-  uint64_t* acc_full = b_empty + MAX_SB;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* l_full = acc_empty + 2;     // UPS: low-res staging ring (2 stages)
+  uint64_t* l_full = b_empty + MAX_SB;     // UPS: low-res staging ring (2 stages)
   uint64_t* l_empty = l_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(l_empty + 2);
   uint8_t* stg_out = smem_b + h.SB * h.b_stage_bytes + 2048;     // TMA-store staging (flat layers), 1024-byte aligned
-  constexpr int W_B = UPS ? UPS_WARP_B : WARP_B, W_MMA = UPS ? UPS_WARP_MMA : WARP_MMA;
+  float* acc_stg = reinterpret_cast<float*>(smem_b + h.SB * h.b_stage_bytes + 1024 + (UPS ? 2 * h.l_stage_bytes : 0) +
+                                            (h.tstore ? 1024 + h.MT * h.out_stage_bytes : 0));
+  constexpr int W_B = UPS ? UPS_WARP_B : WARP_B;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * p.groups;
   const int taps = p.kh * p.kw;
-  const uint32_t set_cols = (uint32_t)(h.MT * h.accw);
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < 2 * set_cols) tmem_cols <<= 1;
 
   if (tid == 0) {
-    for (int s = 0; s < h.SA; ++s) { mbar_init(&a_full[s], UPS ? UPS_INTERP_THREADS : 1); mbar_init(&a_empty[s], 1); }
+    for (int s = 0; s < h.SA; ++s) { mbar_init(&a_full[s], UPS ? UPS_INTERP_THREADS : 1); mbar_init(&a_empty[s], NUM_EPI_THREADS); }
     if (UPS) for (int s = 0; s < 2; ++s) { mbar_init(&l_full[s], 1); mbar_init(&l_empty[s], UPS_INTERP_THREADS); }
-    for (int s = 0; s < h.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], NUM_EPI_THREADS); }
+    for (int s = 0; s < h.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], NUM_EPI_THREADS); }
     mbar_fence_init();
   }
-  if (warp == W_MMA) {
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
+  // 168 registers per thread at launch; the producer warpgroup gives its registers to the accumulator holders (an
+  // increase can only use what this CTA released: 2 x 128 x (232 - 168) == 128 x (168 - 40))
+  if constexpr (!UPS) {
+    if (warp < 8) setmaxnreg_inc<232>();
+    else setmaxnreg_dec<40>();
+  }
   if (warp < 8) {
-    // ------------------------------------------------------------------ epilogue
-    const int quarter = warp & 3, half = warp >> 2;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    const int r = quarter * 32 + lane;          // row of the 128-pixel sub-tile: 16 rows x 8 columns
-    const int epi = p.epi;
-    const bool vec = p.vec_ok != 0;
-    const bool has_aux = p.aux0 != nullptr;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const TileCoord t = decode_tile(h, tile);
-      const int n0 = t.n_idx * p.BN;
-      const int bnt = min(p.BN, p.Cout_g_pad - n0);
-      const int set = it & 1;
-      // MT == 2: warps 0-3 own sub-tile 0, warps 4-7 sub-tile 1.  MT == 1: the two halves split the columns.
-      int sub = 0, c_lo = 0, c_hi = bnt;
-      if (h.MT == 2) sub = half;
-      else {
-        const int split = ((bnt / 16 + 1) / 2) * 16;
-        c_lo = half ? split : 0;
-        c_hi = half ? bnt : split;
-      }
-      bool mvalid;
-      long long mrow;
-      if (h.flat) {
-        mrow = ((long long)t.tx * h.MT + sub) * 128 + r;
-        mvalid = mrow < p.M_total;
-      } else {
-        const int oy = t.ty * 16 + (r >> 3), ox = t.tx * (8 * h.MT) + 8 * sub + (r & 7);
-        mvalid = oy < p.OH && ox < p.OW;
-        mrow = ((long long)t.img * p.OH + oy) * p.OW + ox;
-      }
-      mbar_wait(&acc_full[set], (uint32_t)(it >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + lane_base + set * set_cols + sub * h.accw;
-      const bool skip = !mvalid || (h.debug & 1);
-      // TMA-store path: staging tile of this sub-tile, its barrier (the 4 warps of a sub-tile, or all 8 when MT == 1)
-      uint8_t* stg = nullptr;
-      const int bar_id = 2 + (h.MT == 2 ? half : 0), bar_n = h.MT == 2 ? 128 : 256;
-      const bool issuer = h.MT == 2 ? (tid == half * 128) : (tid == 0);
-      if (h.tstore) {
-        stg = stg_out + sub * h.out_stage_bytes;
-        if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
-        asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
-      }
-      // 32 columns per round: both TMEM loads are in flight before the single wait
-      for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
-        uint32_t raw0[16], raw1[16];
-        const bool two = c0 + 16 < c_hi;
-        tmem_ld16(t_row + c0, raw0);
-        if (two) tmem_ld16(t_row + c0 + 16, raw1);
-        const bool do0 = !skip && n0 + c0 < p.Cout_g, do1 = !skip && two && n0 + c0 + 16 < p.Cout_g;
-        ppconv::EpiAux x0, x1;
-        x0.have = x1.have = false;
-        if (has_aux) {   // residual / GRU operands: issued while the TMEM reads are in flight
-          if (do0) ppconv::conv_epilogue_prefetch16(p, mrow, n0 + c0, epi, vec, x0);
-          if (do1) ppconv::conv_epilogue_prefetch16(p, mrow, n0 + c0 + 16, epi, vec, x1);
-        }
-        tmem_ld_wait();
-        if (c0 + 32 >= c_hi) {   // last read of this accumulator set by this thread: hand it back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(&acc_empty[set]);
-        }
-        if (stg != nullptr) {
-          // 16 columns = two 16-byte units of panel c/64, row r, 128B swizzle (unit index XOR row & 7)
-          auto slot = [&](int c, int u) {
-            const int unit = ((c & 63) >> 3) + u;
-            return reinterpret_cast<uint4*>(stg + (c >> 6) * 16384 + r * 128 + ((unit ^ (r & 7)) << 4));
-          };
-          if (do0) ppconv::conv_epilogue16(p, raw0, mrow, t.g, n0 + c0, epi, vec, &x0, slot(c0, 0), slot(c0, 1));
-          if (do1) ppconv::conv_epilogue16(p, raw1, mrow, t.g, n0 + c0 + 16, epi, vec, &x1, slot(c0 + 16, 0), slot(c0 + 16, 1));
-        } else {
-          if (do0) ppconv::conv_epilogue16(p, raw0, mrow, t.g, n0 + c0, epi, vec, &x0);
-          if (do1) ppconv::conv_epilogue16(p, raw1, mrow, t.g, n0 + c0 + 16, epi, vec, &x1);
-        }
-      }
-      if (c_lo >= c_hi) {
-        tc_fence_before();
-        mbar_arrive(&acc_empty[set]);
-      }
-      if (stg != nullptr) {
-        fence_proxy_async();                                  // generic-proxy smem writes -> visible to the TMA store
-        asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
-        if (issuer && !(h.debug & 1)) {
-          const int row0 = (int)(((long long)t.tx * h.MT + sub) * 128);
-          for (int pnl = 0; pnl * 64 < bnt; ++pnl)
-            tma_store_2d(&h.tmap_out, smem_u32(stg + pnl * 16384), n0 + pnl * 64, row0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-    }
+    // ------------------------------------------------------------------ consumers: wgmma + epilogue
+    const int wg = tid >> 7, t128 = tid & 127;
+    float* stg = acc_stg + wg * (ppconv::STG_BYTES / 4);
+    Ring ra = {0, 0}, rb = {0, 0};
+    auto run = [&](auto bn, auto mb) {
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
+        halo_tile<decltype(bn)::value, decltype(mb)::value>(h, tile, smem, smem_b, h.SA, h.SB, h.a_stage_bytes, h.b_stage_bytes,
+                                                            a_full, a_empty, b_full, b_empty, ra, rb, stg, stg_out, wg, t128);
+    };
+    if constexpr (UPS) ppconv::with_tile_width<128>(p.BN, [&](auto bn) { run(bn, ppconv::IntC<1>{}); });   // MT == 1
+    else with_tile_shape(h.MT, p.BN, run);
     if (h.tstore) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // outstanding stores of this thread complete
   } else if (UPS && warp < 12) {
     // ------------------------------------------------------------------ fused bilinear x2 (align_corners=True) producer
@@ -313,7 +354,7 @@ __global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_
           }
           *reinterpret_cast<uint4*>(dstA + pp * 128 + ((ch ^ (pp & 7)) << 4)) = o;
         }
-        fence_proxy_async();            // generic-proxy writes of the A stage -> visible to tcgen05.mma
+        fence_proxy_async();            // generic-proxy writes of the A stage -> visible to wgmma
         mbar_arrive(&a_full[sa]);
         mbar_arrive(&l_empty[ls]);
         if (++ls == 2) { ls = 0; lph ^= 1; }
@@ -368,75 +409,7 @@ __global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_
         }
       }
     }
-  } else if (warp == W_MMA) {
-    // ------------------------------------------------------------------ MMA issuer
-    // One elected lane (elect.sync lets ptxas emit each tcgen05.mma once instead of a per-lane loop).  The loop is
-    // kept lean -- descriptors advance by precomputed 16-byte-unit steps -- because a single thread has to issue
-    // one UTCHMMA per 32-64 tensor-pipe cycles.
-    if (ppx::elect_one()) {
-      int sa = 0, sb = 0, it = 0;
-      uint32_t pa = 0, pb = 0;
-      const uint32_t sbo = h.flat ? 1024u : (uint32_t)h.BW * 128;
-      const uint64_t a_hi = ((uint64_t)1 << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-      const uint64_t b_hi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-      const uint32_t a_base0 = (smem_u32(smem) & 0x3FFFF) >> 4, b_base0 = (smem_u32(smem_b) & 0x3FFFF) >> 4;
-      const uint32_t a_stage16 = (uint32_t)h.a_stage_bytes >> 4, b_stage16 = (uint32_t)h.b_stage_bytes >> 4;
-      const uint32_t step_x = (uint32_t)p.dw * 8;                                           // next tap in the row
-      const uint32_t step_row = (uint32_t)(p.dh * h.BW - (p.kw - 1) * p.dw) * 8;            // last tap of a row -> next row
-      const uint32_t sub16 = (uint32_t)h.sub_bytes >> 4;
-      const uint32_t tap16 = (uint32_t)p.BN * 8;                                            // next tap's weight tile in the stage
-      const bool two = h.MT == 2;
-      const int kw = p.kw;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int n0 = (tile % h.n_tiles) * p.BN;
-        const uint32_t idesc = umma_idesc_f16(128, (uint32_t)min(p.BN, p.Cout_g_pad - n0));
-        const int set = it & 1;
-        mbar_wait(&acc_empty[set], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + set * set_cols, d1 = d0 + h.accw;
-        uint32_t accum = 0;
-        for (int c = 0; c < h.chunks; ++c) {
-          mbar_wait(&a_full[sa], pa);
-          tc_fence_after();
-          uint64_t adesc = a_hi | (uint64_t)(a_base0 + sa * a_stage16);
-          int kx = 0;
-          for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
-            mbar_wait(&b_full[sb], pb);
-            tc_fence_after();
-            uint64_t bdesc = b_hi | (uint64_t)(b_base0 + sb * b_stage16);
-            const int tn = min(h.tps, taps - tap0);
-            for (int t = 0; t < tn; ++t) {
-              umma_f16(d0, adesc, bdesc, idesc, accum);
-              umma_f16(d0, adesc + 2, bdesc + 2, idesc, 1u);
-              umma_f16(d0, adesc + 4, bdesc + 4, idesc, 1u);
-              umma_f16(d0, adesc + 6, bdesc + 6, idesc, 1u);
-              if (two) {
-                const uint64_t adesc1 = adesc + sub16;
-                umma_f16(d1, adesc1, bdesc, idesc, accum);
-                umma_f16(d1, adesc1 + 2, bdesc + 2, idesc, 1u);
-                umma_f16(d1, adesc1 + 4, bdesc + 4, idesc, 1u);
-                umma_f16(d1, adesc1 + 6, bdesc + 6, idesc, 1u);
-              }
-              accum = 1u;
-              bdesc += tap16;
-              adesc += step_x;
-              if (++kx == kw) { kx = 0; adesc += step_row - step_x; }
-            }
-            umma_commit(&b_empty[sb]);
-            if (++sb == h.SB) { sb = 0; pb ^= 1; }
-          }
-          umma_commit(&a_empty[sa]);
-          if (++sa == h.SA) { sa = 0; pa ^= 1; }
-        }
-        umma_commit(&acc_full[set]);
-      }
-    }
-    __syncwarp();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -445,13 +418,13 @@ __global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_
 // The recurrent propagation steps of flow completion are 8 dependent layers over 3,600-7,200 pixels: as separate
 // launches each pays launch + prologue + pipeline fill/drain (~15-30 us, mostly fixed); here the fixed cost per layer
 // is one barrier (an atomic counter in global memory) and one TMA round trip, the weight producer runs ahead across the
-// barrier, and TMEM / mbarriers / tensor maps are set up once.
+// barrier, and mbarriers / tensor maps are set up once.
 //
-// Ordering between layers: the epilogue threads (the only writers of global memory) make their generic-proxy stores
+// Ordering between layers: the consumer threads (the only writers of global memory) make their generic-proxy stores
 // visible to the async proxy (fence.proxy.async.global), meet on a named barrier, and one thread publishes the CTA's
 // arrival (threadfence + atomicAdd).  The TMA producer and the epilogue warps of the next layer spin on the counter
 // (ld.acquire.gpu) before they touch that layer's inputs; the producer adds the consumer-side proxy fence before
-// issuing TMA loads.  All 148 CTAs are co-resident (1 CTA per SM by shared memory), so the spin cannot deadlock.
+// issuing TMA loads.  All CTAs (one per SM) are co-resident (1 CTA per SM by shared memory), so the spin cannot deadlock.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int PROG_MAX_LAYERS = 10;
 enum { PROG_CONV = 0, PROG_DCN = 1 };
@@ -494,37 +467,28 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
   uint64_t* a_empty = a_full + MAX_SA;
   uint64_t* b_full = a_empty + MAX_SA;
   uint64_t* b_empty = b_full + MAX_SB;
-  uint64_t* acc_full = b_empty + MAX_SB;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* layer_go = acc_empty + 2;     // the CTA's one poller (TMA producer thread) -> epilogue warps: layer li may start
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2 + 4);
+  uint64_t* layer_go = b_empty + MAX_SB;   // the CTA's one poller (TMA producer thread) -> consumers: layer li may start
+  float* acc_stg = reinterpret_cast<float*>(smem_b + P.SB * P.b_stage_bytes + 1024);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const unsigned int G = gridDim.x;
   if (tid == 0) {
     mbar_init(layer_go, 1);
-    for (int s = 0; s < P.SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < P.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], NUM_EPI_THREADS); }
+    for (int s = 0; s < P.SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], NUM_EPI_THREADS); }
+    for (int s = 0; s < P.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], NUM_EPI_THREADS); }
     mbar_fence_init();
   }
-  if (warp == WARP_MMA) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
+  if (warp < 8) setmaxnreg_inc<232>();
+  else setmaxnreg_dec<40>();
   if (warp < 8) {
-    // ------------------------------------------------------------------ epilogue warps (+ the sampling layers)
-    const int quarter = warp & 3, half = warp >> 2;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    const int r = quarter * 32 + lane;
-    int it = 0;
+    // ------------------------------------------------------------------ consumers: wgmma + epilogue (+ the sampling layers)
+    const int wg = tid >> 7, t128 = tid & 127;
+    float* stg = acc_stg + wg * (ppconv::STG_BYTES / 4);
+    Ring ra = {0, 0}, rb = {0, 0};
     for (int li = 0; li < P.n_layers; ++li) {
       // inputs of this layer (residuals, sampling sources) were written by the previous one: the producer thread polls
       // the grid counter for the whole CTA and releases the epilogue warps through a shared-memory barrier
@@ -554,63 +518,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
         }
       } else {
         const HaloParams& h = P.layer[li];
-        const PPConvParams& p = h.c;
-        const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * p.groups;
-        const uint32_t set_cols = (uint32_t)(h.MT * h.accw);
-        const int epi = p.epi;
-        const bool vec = p.vec_ok != 0;
-        const bool has_aux = p.aux0 != nullptr;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += G, ++it) {
-          const TileCoord t = decode_tile(h, tile);
-          const int n0 = t.n_idx * p.BN;
-          const int bnt = min(p.BN, p.Cout_g_pad - n0);
-          const int set = it & 1;
-          int sub = 0, c_lo = 0, c_hi = bnt;
-          if (h.MT == 2) sub = half;
-          else {
-            const int split = ((bnt / 16 + 1) / 2) * 16;
-            c_lo = half ? split : 0;
-            c_hi = half ? bnt : split;
-          }
-          bool mvalid;
-          long long mrow;
-          if (h.flat) {
-            mrow = ((long long)t.tx * h.MT + sub) * 128 + r;
-            mvalid = mrow < p.M_total;
-          } else {
-            const int oy = t.ty * 16 + (r >> 3), ox = t.tx * (8 * h.MT) + 8 * sub + (r & 7);
-            mvalid = oy < p.OH && ox < p.OW;
-            mrow = ((long long)t.img * p.OH + oy) * p.OW + ox;
-          }
-          mbar_wait(&acc_full[set], (uint32_t)(it >> 1) & 1u);
-          tc_fence_after();
-          const uint32_t t_row = tmem_base + lane_base + set * 256u + sub * h.accw;
-          (void)set_cols;
-          for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
-            uint32_t raw0[16], raw1[16];
-            const bool two = c0 + 16 < c_hi;
-            tmem_ld16(t_row + c0, raw0);
-            if (two) tmem_ld16(t_row + c0 + 16, raw1);
-            const bool do0 = mvalid && n0 + c0 < p.Cout_g, do1 = mvalid && two && n0 + c0 + 16 < p.Cout_g;
-            ppconv::EpiAux x0, x1;
-            x0.have = x1.have = false;
-            if (has_aux) {
-              if (do0) ppconv::conv_epilogue_prefetch16(p, mrow, n0 + c0, epi, vec, x0);
-              if (do1) ppconv::conv_epilogue_prefetch16(p, mrow, n0 + c0 + 16, epi, vec, x1);
-            }
-            tmem_ld_wait();
-            if (c0 + 32 >= c_hi) {
-              tc_fence_before();
-              mbar_arrive(&acc_empty[set]);
-            }
-            if (do0) ppconv::conv_epilogue16(p, raw0, mrow, t.g, n0 + c0, epi, vec, &x0);
-            if (do1) ppconv::conv_epilogue16(p, raw1, mrow, t.g, n0 + c0 + 16, epi, vec, &x1);
-          }
-          if (c_lo >= c_hi) {
-            tc_fence_before();
-            mbar_arrive(&acc_empty[set]);
-          }
-        }
+        const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * h.c.groups;
+        // program layers are configured with MT == 1 and BN <= 128 (halo_configure, one_wave): wider or two-sub-tile
+        // instances make this kernel spill its accumulators
+        ppconv::with_tile_width<128>(h.c.BN, [&](auto bn) {
+          for (int tile = blockIdx.x; tile < total_tiles; tile += G)
+            halo_tile<decltype(bn)::value, 1>(h, tile, smem, smem_b, P.SA, P.SB, P.a_stage_bytes, P.b_stage_bytes, a_full,
+                                              a_empty, b_full, b_empty, ra, rb, stg, nullptr, wg, t128);
+        });
       }
       // publish this CTA's part of the layer: stores -> async proxy, CTA-wide meet of the writers, one arrival
       fence_proxy_async_global();
@@ -691,79 +606,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
         }
       }
     }
-  } else if (warp == WARP_MMA) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (ppx::elect_one()) {
-      int sa = 0, sb = 0, it = 0;
-      uint32_t pa = 0, pb = 0;
-      const uint64_t b_hi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-      const uint32_t a_base0 = (smem_u32(smem) & 0x3FFFF) >> 4, b_base0 = (smem_u32(smem_b) & 0x3FFFF) >> 4;
-      const uint32_t a_stage16 = (uint32_t)P.a_stage_bytes >> 4, b_stage16 = (uint32_t)P.b_stage_bytes >> 4;
-      for (int li = 0; li < P.n_layers; ++li) {
-        if (P.kind[li] != PROG_CONV) continue;
-        const HaloParams& h = P.layer[li];
-        const PPConvParams& p = h.c;
-        const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * p.groups;
-        const int taps = p.kh * p.kw;
-        const uint32_t sbo = h.flat ? 1024u : (uint32_t)h.BW * 128;
-        const uint64_t a_hi = ((uint64_t)1 << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-        const uint32_t step_x = (uint32_t)p.dw * 8;
-        const uint32_t step_row = (uint32_t)(p.dh * h.BW - (p.kw - 1) * p.dw) * 8;
-        const uint32_t sub16 = (uint32_t)h.sub_bytes >> 4;
-        const uint32_t tap16 = (uint32_t)p.BN * 8;
-        const bool two = h.MT == 2;
-        const int kw = p.kw;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += G, ++it) {
-          const int n0 = (tile % h.n_tiles) * p.BN;
-          const uint32_t idesc = umma_idesc_f16(128, (uint32_t)min(p.BN, p.Cout_g_pad - n0));
-          const int set = it & 1;
-          mbar_wait(&acc_empty[set], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          const uint32_t d0 = tmem_base + set * 256u, d1 = d0 + h.accw;
-          uint32_t accum = 0;
-          for (int c = 0; c < h.chunks; ++c) {
-            mbar_wait(&a_full[sa], pa);
-            tc_fence_after();
-            uint64_t adesc = a_hi | (uint64_t)(a_base0 + sa * a_stage16);
-            int kx = 0;
-            for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
-              mbar_wait(&b_full[sb], pb);
-              tc_fence_after();
-              uint64_t bdesc = b_hi | (uint64_t)(b_base0 + sb * b_stage16);
-              const int tn = min(h.tps, taps - tap0);
-              for (int t = 0; t < tn; ++t) {
-                umma_f16(d0, adesc, bdesc, idesc, accum);
-                umma_f16(d0, adesc + 2, bdesc + 2, idesc, 1u);
-                umma_f16(d0, adesc + 4, bdesc + 4, idesc, 1u);
-                umma_f16(d0, adesc + 6, bdesc + 6, idesc, 1u);
-                if (two) {
-                  const uint64_t adesc1 = adesc + sub16;
-                  umma_f16(d1, adesc1, bdesc, idesc, accum);
-                  umma_f16(d1, adesc1 + 2, bdesc + 2, idesc, 1u);
-                  umma_f16(d1, adesc1 + 4, bdesc + 4, idesc, 1u);
-                  umma_f16(d1, adesc1 + 6, bdesc + 6, idesc, 1u);
-                }
-                accum = 1u;
-                bdesc += tap16;
-                adesc += step_x;
-                if (++kx == kw) { kx = 0; adesc += step_row - step_x; }
-              }
-              umma_commit(&b_empty[sb]);
-              if (++sb == P.SB) { sb = 0; pb ^= 1; }
-            }
-            umma_commit(&a_empty[sa]);
-            if (++sa == P.SA) { sa = 0; pa ^= 1; }
-          }
-          umma_commit(&acc_full[set]);
-        }
-      }
-    }
-    __syncwarp();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_MMA) tmem_dealloc(tmem_base, 512);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -839,7 +682,7 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   int num_sms = 0;
   PP_TRY(halo_num_sms(&num_sms));
   const bool flat = p.kh * p.kw == 1;
-  // N tile: <= 128 columns (two accumulator sets x two sub-tiles fill the 512 TMEM columns)
+  // N tile: <= 128 columns (MT x BN accumulators of a consumer warpgroup stay within 128 registers per thread)
   const int n_tiles0 = pp_ceil_div(p.Cout_g_pad, 128);
   int bn = pp_ceil_div(pp_ceil_div(p.Cout_g_pad, n_tiles0), 16) * 16;
   const int tiles_y = flat ? 1 : pp_ceil_div(p.OH, 16);
@@ -848,16 +691,19 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   auto count = [&](int mt, int bn_) {
     return (long long)pp_ceil_div(p.Cout_g_pad, bn_) * tiles_x(mt) * tiles_y * n_img * p.groups;
   };
+  // fused-upsample layers run 416 threads (at most 157 registers each): one sub-tile per CTA keeps the accumulators small
   int mt = 2;
-  if (!p.ups2x && count(2, bn) < num_sms) mt = 1;
+  if (p.ups2x || count(2, bn) < num_sms) mt = 1;
   while (count(mt, bn) < num_sms && bn >= 64 && bn % 32 == 0) bn /= 2;   // small launches: more, narrower tiles
   if (one_wave && !p.ups2x) {
-    // largest tile count that still fits one wave: 128-pixel tiles, N split into 1..8 tiles of <= 256 columns
+    // largest tile count that still fits one wave: 128-pixel tiles, N split into 1..8 tiles of <= 128 columns (the
+    // only shapes the program kernel instantiates; the fallback bn above is <= 128 too)
+    mt = 1;
     static int min_bn = -1;
     if (min_bn < 0) { const char* e = getenv("PP_PROG_MIN_BN"); min_bn = e != nullptr ? atoi(e) : 16; }
     for (int nt = 8; nt >= 1; --nt) {
       const int b = pp_ceil_div(pp_ceil_div(p.Cout_g_pad, nt), 16) * 16;
-      if (b > 256 || b < 16 || (b < min_bn && nt > 1)) continue;
+      if (b > 128 || b < 16 || (b < min_bn && nt > 1)) continue;
       if (count(1, b) <= num_sms) { mt = 1; bn = b; break; }
     }
   }
@@ -872,7 +718,6 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   h.tiles_y = tiles_y;
   h.n_tiles = pp_ceil_div(p.Cout_g_pad, bn);
   h.chunks = pp_ceil_div(p.Cin, 64);
-  h.accw = pp_ceil_div(bn, 32) * 32;
   h.a_stage_bytes = pp_ceil_div(h.BW * h.BH * 128, 1024) * 1024;
   {
     // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloParams::tps
@@ -976,8 +821,8 @@ int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   int num_sms = 0;
   PP_TRY(halo_num_sms(&num_sms));
   const long long total_tiles = halo_total_tiles(h);
-  const size_t smem = (size_t)h.SA * h.a_stage_bytes + (size_t)h.SB * h.b_stage_bytes + 1024 + 512 + 2 * (size_t)h.l_stage_bytes +
-                      (h.ups ? 1024 : 0) + (h.tstore ? (size_t)h.MT * h.out_stage_bytes + 1536 : 0);
+  const size_t smem = (size_t)h.SA * h.a_stage_bytes + (size_t)h.SB * h.b_stage_bytes + 1024 + 1024 + 2 * (size_t)h.l_stage_bytes +
+                      (h.tstore ? (size_t)h.MT * h.out_stage_bytes + 1024 : 0) + 2 * ppconv::STG_BYTES;
   const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -1030,6 +875,8 @@ int pp_prog_record_conv(const PPConvParams& p) {
   PP_REQUIRE(pp_prog_eligible(p), "conv program: layer is not a stride-1 TMA halo-kernel convolution");
   const int li = r->prog.n_layers;
   PP_TRY(halo_configure(p, r->prog.layer[li], true));
+  PP_REQUIRE(r->prog.layer[li].MT == 1 && r->prog.layer[li].c.BN <= 128, "conv program: layer tile %d x %d columns",
+             r->prog.layer[li].MT, r->prog.layer[li].c.BN);
   r->prog.kind[li] = PROG_CONV;
   r->prog.n_layers++;
   r->n_conv++;
@@ -1084,7 +931,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
   P.ts = (ts_mode && ts_printed < ts_mode) ? ts_dev : nullptr;
   const int grid = num_sms;
   *arrivals += (unsigned int)(P.n_layers * grid);
-  const size_t smem = (size_t)sa * a_max + (size_t)sb * b_max + 1024 + 512;
+  const size_t smem = (size_t)sa * a_max + (size_t)sb * b_max + 1024 + 1024 + 2 * ppconv::STG_BYTES;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);

@@ -1,13 +1,12 @@
-// tcgen05 implicit-GEMM convolution for sm_100a.  See conv_igemm.cuh for the contract.
+// wgmma implicit-GEMM convolution for sm_90a.  See conv_igemm.cuh for the contract.
 //
-// Persistent CTA (one per SM, 448 threads) looping over 128 x BN output tiles:
-//   warps 0-3   epilogue: tcgen05.ld of the finished accumulator -> bias/activation/fusions -> global
-//   warps 4-11  im2col producers: 16-byte cp.async gathers into a 128B-swizzled K-major A tile
-//   warp  12    one lane issues tcgen05.mma (M=128, N=BN, K=16 x4 per 64-wide K chunk)
-//   warp  13    TMEM allocation; one lane streams the pre-swizzled weight tile with a single
-//               cp.async.bulk (TMA engine) per stage
-// Pipelines: `stages` smem slots (full/empty mbarriers) that keep filling across tile boundaries, and two
-// TMEM accumulators (acc_full/acc_empty) so the epilogue of tile i overlaps the main loop of tile i+1.
+// Persistent CTA (one per SM, 384 threads) looping over 128 x BN output tiles:
+//   warpgroups 0-1  consumers: warpgroup w issues wgmma (M=64 rows 64w.., N=BN, K=16 x4 per 64-wide K chunk) into
+//                   register accumulators, then runs the fused epilogue of its 64 rows (conv_epilogue.cuh)
+//   warpgroup 2     im2col producers: 16-byte cp.async gathers into a 128B-swizzled K-major A tile; thread 0 also
+//                   streams the pre-swizzled weight tile with a single cp.async.bulk (TMA engine) per stage
+// Pipeline: `stages` smem slots (full/empty mbarriers) that keep filling across tile boundaries, so the producers run
+// ahead through the consumers' epilogue.
 #include <string.h>
 
 #include "conv_igemm.cuh"
@@ -18,13 +17,56 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KiB
-constexpr int NUM_EPILOGUE = 128;   // warps 0-3
-constexpr int NUM_PRODUCERS = 256;  // warps 4-11
-constexpr int WARP_MMA = 12;
-constexpr int WARP_TMA = 13;
-constexpr int NUM_THREADS = 448;
+constexpr int NUM_CONSUMERS = 256;  // warpgroups 0-1
+constexpr int NUM_PRODUCERS = 128;  // warpgroup 2
+constexpr int NUM_THREADS = 384;
 constexpr int MAX_STAGES = 8;
-constexpr int SMEM_BUDGET = 200 * 1024;
+constexpr int SMEM_BUDGET = 192 * 1024;
+
+template <int BN>
+__device__ __forceinline__ void igemm_consume(const PPConvParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
+                                              uint64_t* empty_bar, float* stg, int wg, int t128) {
+  using namespace ppx;
+  const int S = p.stages;
+  const int num_kc = p.num_kc;
+  const int m_tiles = (p.M_total + BM - 1) / BM;
+  const int n_tiles = p.Cout_g_pad / p.BN;
+  const int total_tiles = m_tiles * n_tiles * p.groups;
+  float acc[BN / 2];
+  int s = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int n_idx = tile % n_tiles;
+    const int rest = tile / n_tiles;
+    const int m0 = (rest % m_tiles) * BM;
+    const int g = rest / m_tiles;
+    const int n0 = n_idx * p.BN;
+    int prev = -1;
+    for (int kc = 0; kc < num_kc; ++kc) {
+      mbar_wait(&full_bar[s], phase);
+      fence_proxy_async();   // the A tile was written by cp.async (generic proxy)
+      wgmma_fence();
+      const uint32_t a_addr = smem_u32(smem + s * stage_bytes);
+      const uint64_t adesc = gmma_desc_sw128_kmajor(a_addr + wg * (A_STAGE_BYTES / 2));
+      const uint64_t bdesc = gmma_desc_sw128_kmajor(a_addr + A_STAGE_BYTES);
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) wgmma_f16<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kc | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous chunk's MMAs are done: its slot may be refilled
+      if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+      prev = s;
+      if (++s == S) { s = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    mbar_arrive(&empty_bar[prev]);
+    ppconv::drain_acc<BN>(acc, stg, t128, 4 + wg, [&](const float* src, int r, int c) {
+      const int m = m0 + wg * 64 + r;
+      if (m < p.M_total && n0 + c < p.Cout_g)
+        ppconv::epilogue_from_stage(p, src, m, g, n0 + c, nullptr, nullptr);
+    });
+  }
+}
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid_constant__ PPConvParams p) {
   using namespace ppx;
@@ -35,98 +77,58 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
   const int S = p.stages;
   const int b_stage_bytes = p.BN * 128;
   const int stage_bytes = A_STAGE_BYTES + b_stage_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * stage_bytes);
+  float* stg = reinterpret_cast<float*>(smem + S * stage_bytes);     // 2 x STG_BYTES accumulator staging
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * stage_bytes + 2 * ppconv::STG_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;   // [2] accumulator ready for the epilogue
-  uint64_t* acc_empty = acc_full + 2;            // [2] accumulator drained, MMA may overwrite
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
   const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const int lane = tid & 31;
   const int num_kc = p.num_kc;
   const int m_tiles = (p.M_total + BM - 1) / BM;
   const int n_tiles = p.Cout_g_pad / p.BN;
   const int total_tiles = m_tiles * n_tiles * p.groups;
 
-  // two accumulator buffers of `acc_cols` TMEM columns each
-  uint32_t acc_cols = 32;
-  while (acc_cols < (uint32_t)p.BN) acc_cols <<= 1;
-  const uint32_t tmem_cols = acc_cols * 2;
-
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], NUM_PRODUCERS + 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], NUM_EPILOGUE);
+      mbar_init(&empty_bar[s], NUM_CONSUMERS);
     }
     mbar_fence_init();
   }
-  if (warp == WARP_TMA) {
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation) overlapped the tail of the
-  // previous kernel in the stream; from here on we read its outputs.  Let our own dependents start their prologue.
+  // Programmatic dependent launch: everything above (barrier init) overlapped the tail of the previous kernel in the
+  // stream; from here on we read its outputs.  Let our own dependents start their prologue.
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp < 4) {
-    // ------------------------------------------------------------------ epilogue warps (TMEM lanes 32*warp..)
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    const int epi = p.epi;
-    const bool vec = p.vec_ok != 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int n_idx = tile % n_tiles;
-      const int rest = tile / n_tiles;
-      const int m0 = (rest % m_tiles) * BM;
-      const int g = rest / m_tiles;
-      const int n0 = n_idx * p.BN;
-      const int buf = it & 1;
-      mbar_wait(&acc_full[buf], (uint32_t)(it >> 1) & 1u);
-      tc_fence_after();
-      const int m = m0 + warp * 32 + lane;
-      const bool mvalid = m < p.M_total;
-      const uint32_t t_row = tmem_base + lane_base + buf * acc_cols;
-      const long long mrow = m;
-      for (int c0 = 0; c0 < p.BN; c0 += 16) {
-        uint32_t raw[16];
-        tmem_ld16(t_row + c0, raw);
-        tmem_ld_wait();
-        if (c0 + 16 >= p.BN) {  // last read of this accumulator: hand the buffer back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(&acc_empty[buf]);
-        }
-        const int ng0 = n0 + c0;  // channel within the group
-        if (!mvalid || ng0 >= p.Cout_g) continue;
-        ppconv::conv_epilogue16(p, raw, mrow, g, ng0, epi, vec);
-      }
-    }
-  } else if (warp < WARP_MMA) {
-    // ------------------------------------------------------------------ im2col producers (8 warps)
-    const int ptid = tid - 128;
+  // 168 registers per thread at launch; the producers give theirs to the accumulator-holding consumers.  An increase
+  // can only use what this CTA's warpgroups released: 2 x 128 x (216 - 168) <= 128 x (168 - 64).
+  if (tid < NUM_CONSUMERS) {
+    setmaxnreg_inc<216>();
+    const int wg = tid >> 7;
+    ppconv::with_tile_width<256>(p.BN, [&](auto bn) {
+      igemm_consume<decltype(bn)::value>(p, smem, stage_bytes, full_bar, empty_bar, stg + wg * (ppconv::STG_BYTES / 4), wg,
+                                         tid & 127);
+    });
+  } else {
+    // ------------------------------------------------------------------ im2col producers (+ weight tile loader)
+    setmaxnreg_dec<64>();
+    const int ptid = tid - NUM_CONSUMERS;
     const int j = ptid & 7;    // 16-byte chunk inside the 128-byte K row
-    const int rb = ptid >> 3;  // rows rb, rb+32, rb+64, rb+96
+    const int rb = ptid >> 3;  // rows rb, rb+16, ..., rb+112
     const uint32_t a_off = rb * 128 + ((j ^ (rb & 7)) << 4);
     int s = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int n0 = (tile % n_tiles) * p.BN;
       const int rest = tile / n_tiles;
       const int m0 = (rest % m_tiles) * BM;
       const int g = rest / m_tiles;
-      int rpix[4], riy[4], rix[4];
+      const __half* wsrc = p.wpacked + ((long long)g * num_kc * p.Cout_g_pad + n0) * BK;
+      int rpix[8], riy[8], rix[8];
       uint32_t rvalid = 0;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int m = m0 + rb + 32 * i;
+      for (int i = 0; i < 8; ++i) {
+        const int m = m0 + rb + 16 * i;
         if (m < p.M_total) {
           const int ox = m % p.OW;
           const int t = m / p.OW;
@@ -148,6 +150,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
       int kx = tap0 - ky * p.kw;
       for (int kc = 0; kc < num_kc; ++kc) {
         mbar_wait(&empty_bar[s], phase ^ 1);
+        if (ptid == 0) {
+          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)b_stage_bytes);
+          bulk_g2s(smem_u32(smem + s * stage_bytes + A_STAGE_BYTES), wsrc + (long long)kc * p.Cout_g_pad * BK,
+                   (uint32_t)b_stage_bytes, &full_bar[s]);
+        }
         const bool kvalid = k < p.K_total;
         int q = 0;
 #pragma unroll
@@ -158,7 +165,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
         const int dy = ky * p.dh, dx = kx * p.dw;
         const uint32_t a_dst = smem_u32(smem + s * stage_bytes) + a_off;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < 8; ++i) {
           int iy = riy[i] + dy, ix = rix[i] + dx;
           bool v = kvalid && ((rvalid >> i) & 1u);
           if (p.pad_replicate) {
@@ -168,7 +175,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
             v = v && ((unsigned)iy < (unsigned)p.H) && ((unsigned)ix < (unsigned)p.W);
           }
           const __half* src = v ? sbase + (long long)(rpix[i] + iy * p.W + ix) * cs : p.seg[0].ptr;
-          cp_async16(a_dst + i * (32 * 128), src, v ? 16u : 0u);
+          cp_async16(a_dst + i * (16 * 128), src, v ? 16u : 0u);
         }
         k += BK;
         ci += BK;
@@ -182,57 +189,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
         if (++s == S) { s = 0; phase ^= 1; }
       }
     }
-  } else if (warp == WARP_MMA) {
-    // ------------------------------------------------------------------ MMA issuer (elect.sync: one UTCHMMA
-    // per tcgen05.mma instead of ptxas' per-lane loop around a uniform-datapath instruction)
-    if (elect_one()) {
-      const uint32_t idesc = umma_idesc_f16(BM, p.BN);
-      int s = 0, it = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&acc_empty[buf], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_addr = tmem_base + buf * acc_cols;
-        for (int kc = 0; kc < num_kc; ++kc) {
-          mbar_wait(&full_bar[s], phase);
-          tc_fence_after();
-          fence_proxy_async();
-          const uint32_t a_addr = smem_u32(smem + s * stage_bytes);
-          const uint64_t adesc = umma_desc_sw128_kmajor(a_addr);
-          const uint64_t bdesc = umma_desc_sw128_kmajor(a_addr + A_STAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_f16(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, (kc | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[s]);
-          if (++s == S) { s = 0; phase ^= 1; }
-        }
-        umma_commit(&acc_full[buf]);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ weight-tile loader (TMA bulk copy)
-    if (elect_one()) {
-      int s = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int n0 = (tile % n_tiles) * p.BN;
-        const int g = tile / (n_tiles * m_tiles);
-        const __half* wsrc = p.wpacked + ((long long)g * num_kc * p.Cout_g_pad + n0) * BK;
-        for (int kc = 0; kc < num_kc; ++kc) {
-          mbar_wait(&empty_bar[s], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)b_stage_bytes);
-          bulk_g2s(smem_u32(smem + s * stage_bytes + A_STAGE_BYTES), wsrc + (long long)kc * p.Cout_g_pad * BK,
-                   (uint32_t)b_stage_bytes, &full_bar[s]);
-          if (++s == S) { s = 0; phase ^= 1; }
-        }
-      }
-    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_TMA) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 }  // namespace
@@ -270,13 +227,6 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
     if (p.bias != nullptr) ok = ok && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0 && (p.groups == 1 || p.Cout_g % 4 == 0);
     if (p.epi == PP_EPI_GRU_ZR) ok = ok && ((p.Cout_g >> 1) % 16 == 0);
     p.vec_ok = ok ? 1 : 0;
-    auto al32 = [](const void* ptr, long long cs, long long co, long long gs) {
-      return ptr == nullptr || ((reinterpret_cast<uintptr_t>(ptr) & 31) == 0 && cs % 16 == 0 && co % 16 == 0 && gs % 16 == 0);
-    };
-    p.vec32_ok = (ok && !p.out_fp32 && al32(p.out, p.out_cstride, p.out_coff, p.out_gstep) &&
-                  al32(p.aux0, p.aux0_cstride, p.aux0_coff, 0) && al32(p.aux1, p.aux1_cstride, p.aux1_coff, 0) &&
-                  al32(p.out2, p.out2_cstride, p.out2_coff, 0) && (p.epi != PP_EPI_GRU_ZR || ((p.Cout_g >> 1) % 16 == 0)))
-                     ? 1 : 0;
   }
   if (pp_prog_recording()) { g_last_kind = 'p'; return pp_prog_record_conv(p); }
   if (pp_conv_halo_eligible(p)) { g_last_kind = 'h'; return pp_launch_conv_halo(p, stream); }
@@ -289,7 +239,7 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   int stages = SMEM_BUDGET / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   p.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + 1024 + 256;
+  const size_t smem = (size_t)stages * stage_bytes + 2 * ppconv::STG_BYTES + 1024 + 256;
   static int num_sms = 0;
   if (num_sms == 0) {
     int dev = 0;

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear layer on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution / linear layer on Hopper tensor cores (wgmma, sm_90a).
 //
 //   out[m][n] = epilogue( sum_k A[m][k] * Wt[n][k] + bias[n] )
 //   m = (image, oy, ox) flattened, n = output channel, k = (ky, kx, ci)
@@ -45,7 +45,6 @@ struct PPConvParams {
   int Cout_g, Cout_g_pad, BN, groups;
   int stages;
   int vec_ok;             // set by the launcher: every epilogue pointer/stride allows 16-byte accesses on full runs
-  int vec32_ok;           // ... and fp16 epilogue operands are 32-byte aligned: one 256-bit access per 16 channels
   // epilogue
   int epi, act1, act2;
   float slope, scale;

@@ -47,8 +47,6 @@ __device__ __forceinline__ void dcn_sample_item(const PPDcnArgs& a, unsigned idx
   float acc[CPG];
 #pragma unroll
   for (int i = 0; i < CPG; ++i) acc[i] = 0.f;
-  const bool wide_st = ((reinterpret_cast<uintptr_t>(a.cols) | (uintptr_t)(C * 2)) & 31) == 0;   // 32-byte aligned rows
-  bool wide = false;
   if (py > -1.f && py < (float)H && px > -1.f && px < (float)W) {
     const float fy = floorf(py), fx = floorf(px);
     const int y0 = (int)fy, xx0 = (int)fx;
@@ -59,7 +57,6 @@ __device__ __forceinline__ void dcn_sample_item(const PPDcnArgs& a, unsigned idx
     if (c < a.C0) { src = a.x0 + a.x0_co + c; cs = a.x0_cs; }
     else { src = a.x1 + a.x1_co + (c - a.C0); cs = a.x1_cs; }
     src += (long long)n * H * W * cs;
-    wide = ((reinterpret_cast<uintptr_t>(src) | (uintptr_t)(cs * 2)) & 31) == 0;
 #pragma unroll
     for (int corner = 0; corner < 4; ++corner) {
       const int yy = y0 + (corner >> 1), xx = xx0 + (corner & 1);
@@ -67,17 +64,8 @@ __device__ __forceinline__ void dcn_sample_item(const PPDcnArgs& a, unsigned idx
       const float w = ((corner >> 1) ? ay : 1.f - ay) * ((corner & 1) ? ax : 1.f - ax);
       const uint4* vp = reinterpret_cast<const uint4*>(src + ((long long)yy * W + xx) * cs);
       uint4 qv[CPG / 8];
-      if (CPG == 16 && wide) {
-        // one 256-bit request per corner (sm_100 LDG.256): the sampler is bound by L1 wavefronts, one per uncoalesced
-        // request, so 32 bytes in one request halve its dominant cost.  .cg = L2 only (COHERENT and not differ only in L1)
-        asm volatile("ld.global.cg.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(qv[0].x), "=r"(qv[0].y), "=r"(qv[0].z), "=r"(qv[0].w), "=r"(qv[CPG / 8 - 1].x), "=r"(qv[CPG / 8 - 1].y),
-                       "=r"(qv[CPG / 8 - 1].z), "=r"(qv[CPG / 8 - 1].w)
-                     : "l"(vp));
-      } else {
 #pragma unroll
-        for (int v = 0; v < CPG / 8; ++v) qv[v] = COHERENT ? __ldcg(vp + v) : vp[v];
-      }
+      for (int v = 0; v < CPG / 8; ++v) qv[v] = COHERENT ? __ldcg(vp + v) : vp[v];
 #pragma unroll
       for (int v = 0; v < CPG / 8; ++v) {
         const __half2* hq = reinterpret_cast<const __half2*>(&qv[v]);
@@ -91,18 +79,11 @@ __device__ __forceinline__ void dcn_sample_item(const PPDcnArgs& a, unsigned idx
     }
   }
   __half* d = a.cols + m * (long long)(9 * C) + k * C + g * CPG;
-  __align__(32) __half2 h[CPG / 2];
+  __align__(16) __half2 h[CPG / 2];
 #pragma unroll
   for (int e = 0; e < CPG / 2; ++e) h[e] = __floats2half2_rn(mod * acc[2 * e], mod * acc[2 * e + 1]);
-  if (CPG == 16 && wide_st) {
-    const uint4 s0 = reinterpret_cast<uint4*>(h)[0], s1 = reinterpret_cast<uint4*>(h)[CPG / 8 - 1];
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(d), "r"(s0.x), "r"(s0.y), "r"(s0.z), "r"(s0.w),
-                 "r"(s1.x), "r"(s1.y), "r"(s1.z), "r"(s1.w)
-                 : "memory");
-  } else {
 #pragma unroll
-    for (int v = 0; v < CPG / 8; ++v) reinterpret_cast<uint4*>(d)[v] = reinterpret_cast<uint4*>(h)[v];
-  }
+  for (int v = 0; v < CPG / 8; ++v) reinterpret_cast<uint4*>(d)[v] = reinterpret_cast<uint4*>(h)[v];
 }
 
 

@@ -355,7 +355,7 @@ int pp_stage_gen_run(PPEngine& e, const int* frame_ids, const int* win_t, const 
     PP_CUDA_CHECK(cudaStreamSynchronize(st));
   }
 
-  // gather table scratch of the tcgen05 attention kernel: [5x9 windows][keys of a masked window]
+  // gather table scratch of the wgmma attention kernel: [5x9 windows][keys of a masked window]
   const int key_stride = ((t_max + 1) / 2) * (193 + np);
   int* key_tab;
   PP_TRY(pp_alloc(e, &key_tab, (size_t)(nh / WIN_H) * (nw / WIN_W) * key_stride, "attention key table"));

@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(256) instnorm_apply(const __half* __restrict__
 
 // ------------------------------------------------------------------------------------------------
 // Pack a row-major [G][R][K] fp16 matrix into the swizzled B-operand tile image consumed by the
-// tcgen05 GEMM ([G][K/64][R_pad] rows of 128 B, 16-byte chunk index XOR (row & 7)); rows >= R are zero.
+// wgmma GEMM ([G][K/64][R_pad] rows of 128 B, 16-byte chunk index XOR (row & 7)); rows >= R are zero.
 // Used for the all-pairs correlation, where fmap2 plays the role of the weights (RAFT/corr.py:52-60).
 // ------------------------------------------------------------------------------------------------
 __global__ void pack_b_operand(const __half* __restrict__ src, __half* __restrict__ dst, int R, int R_pad, int K,

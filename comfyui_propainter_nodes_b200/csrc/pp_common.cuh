@@ -1,5 +1,5 @@
-// Shared device/host helpers for the sm_100a ProPainter kernels.
-// PTX wrappers for mbarrier, cp.async, bulk async copy (TMA engine) and tcgen05 (MMA/TMEM).
+// Shared device/host helpers for the sm_90a ProPainter kernels.
+// PTX wrappers for mbarrier, cp.async, bulk async copy (TMA engine) and wgmma.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -140,7 +140,7 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-// generic-proxy writes -> visible to the async proxy (tcgen05.mma / TMA reads of shared memory)
+// generic-proxy writes -> visible to the async proxy (wgmma / TMA reads of shared memory)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // Bulk async copy global -> shared through the TMA engine (SASS: UBLKCP), completion on an mbarrier.
@@ -151,97 +151,50 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
+// ------------------------------------------------------------------ wgmma (warpgroup MMA, accumulators in registers)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// keeps the compiler from touching accumulator registers across a wgmma_wait
+template <int N>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// Accumulator fragment of m64nNk16 (fp32): register i of thread t of the warpgroup holds
+//   row 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),  column 8 * (i / 4) + 2 * (t % 4) + i % 2.
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp reads TMEM lane (lane_base + t).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, K-major operand tile stored as rows of 64 fp16 (128 B) with the
-// 128-byte swizzle (16-byte chunk index XOR (row & 7)); 8-row groups are 1024 B apart (SBO).
-// Field layout follows cute::UMMA::SmemDescriptor (cute/arch/mma_sm100_desc.hpp).
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
+// Shared-memory matrix descriptor (wgmma), 128-byte swizzle (16-byte chunk index XOR address bits 7-9), so a view
+// that starts at any 128-byte row of a swizzled tile reads what TMA / the producers wrote there.
+// K-major tile: rows of 64 fp16 (128 B); `sbo` = bytes between 8-row groups (1024 for a dense tile).
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address, 16-byte units
-  d |= (uint64_t)1 << 16;                       // leading byte offset (ignored for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);       // start address, 16-byte units
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;        // leading byte offset
+  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;        // stride byte offset
+  d |= (uint64_t)1 << 62;                            // SWIZZLE_128B
   return d;
 }
-
-// MN-major B operand ([K rows][64 N-elements] panels of 128-byte rows, 128B swizzle, e.g. V[key][d] for P.V):
+__device__ __forceinline__ uint64_t gmma_desc_sw128_kmajor(uint32_t smem_addr, uint32_t sbo = 1024) {
+  return gmma_desc_sw128(smem_addr, 16, sbo);        // LBO unused for swizzled K-major
+}
+// MN-major B operand ([K rows][64 N-elements] panels of 128-byte rows, e.g. V[key][d] for P.V):
 // 8-row K groups are 1024 B apart (SBO), consecutive 64-element N panels are `panel_bytes` apart (LBO).
-__device__ __forceinline__ uint64_t umma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t panel_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((panel_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+__device__ __forceinline__ uint64_t gmma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t panel_bytes) {
+  return gmma_desc_sw128(smem_addr, panel_bytes, 1024);
 }
 
-// Instruction descriptor for kind::f16: fp16 A/B (K-major both), fp32 accumulate, M=128, N=n.
-__device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t m, uint32_t n) {
-  uint32_t d = 0;
-  d |= 1u << 4;          // D format F32
-  d |= 0u << 7;          // A format F16
-  d |= 0u << 10;         // B format F16
-  d |= (n >> 3) << 17;   // N / 8
-  d |= (m >> 4) << 24;   // M / 16
-  return d;
-}
-// same with the B operand MN-major (bit 16)
-__device__ __forceinline__ uint32_t umma_idesc_f16_bmn(uint32_t m, uint32_t n) { return umma_idesc_f16(m, n) | (1u << 16); }
+// warpgroup-wide register reallocation (all threads of the warpgroup execute it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// named barrier over `n` threads (multiple of 32)
+__device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // true on exactly one lane of the (converged) warp
 __device__ __forceinline__ bool elect_one() {

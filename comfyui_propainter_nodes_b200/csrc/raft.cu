@@ -148,7 +148,7 @@ int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int ite
 
   // Both directions share one batch: pair slot s < npairs is the forward pair (s -> s+1), slot npairs + s the backward
   // pair (s+1 -> s).  One launch per layer then covers 2(T-1) pairs (half as many launches and tile-quantisation
-  // tails on the 148 SMs as one batch per direction); only the steps that address frames (correlation, context
+  // tails on the SMs as one batch per direction); only the steps that address frames (correlation, context
   // split, final upsampling) run once per direction sub-range of the batch.
   struct Sub { int dir, b0, cnt, off; };   // direction, first pair of that direction, count, slot offset in the batch
   for (int s0 = 0; s0 < 2 * npairs; s0 += max_pairs) {

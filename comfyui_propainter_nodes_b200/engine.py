@@ -1,8 +1,8 @@
-"""ctypes binding of libpropainter_b200.so + checkpoint packing for the sm_100a kernels.
+"""ctypes binding of libpropainter_b200.so + checkpoint packing for the sm_90a kernels.
 
 PyTorch is used here only for device memory, streams and host-side weight re-layout; every compute
 step goes through the C ABI declared in include/propainter_b200.h.  There is NO fallback path: if the
-shared library is missing or the device is not a B200, construction fails loudly.
+shared library is missing or the device is not an H100 (sm_90), construction fails loudly.
 """
 from __future__ import annotations
 
@@ -92,9 +92,9 @@ def exported_symbols():
 
 
 def choose_bn(cout: int) -> Tuple[int, int]:
-    """N-tile of the tcgen05 GEMM: tiles of <= MAX_BN columns (multiple of 16) with the least padding.
+    """N-tile of the wgmma GEMM: tiles of <= MAX_BN columns (multiple of 16) with the least padding.
 
-    MAX_BN = 256: two 256-column fp32 accumulators fill the 512 TMEM columns of the persistent CTA, and a wide
+    MAX_BN = 256: a 64 x 256 fp32 accumulator is 128 registers per consumer thread, and a wide
     N tile halves the im2col (A operand) traffic per output for the Cout >= 256 layers."""
     best = None
     t0 = (cout + MAX_BN - 1) // MAX_BN
@@ -114,7 +114,7 @@ def pack_conv_weight(w: torch.Tensor, groups: int = 1, cin_map=None):
     K is ordered (ky, kx, ci) with ci running over the *kernel's* input channels: ``cin_map[ci]`` is
     the reference input channel feeding kernel channel ci, or -1 for a zero (padding) channel.
     Layout: [groups][K_pad/64][cout_g_pad] rows of 64 fp16; inside each 128-byte row the 16-byte chunk
-    c is stored at position c ^ (row & 7) (the 128B swizzle the UMMA descriptor expects)."""
+    c is stored at position c ^ (row & 7) (the 128B swizzle the wgmma descriptor expects)."""
     w = w.detach().float().cpu()
     cout, cin_ref, kh, kw = w.shape
     if cin_map is None:
@@ -305,7 +305,7 @@ class Engine:
         self.lib = load_library()
         self.device = torch.device(device)
         if self.device.type != "cuda" or not torch.cuda.is_available():
-            raise RuntimeError("the ProPainter B200 engine needs a CUDA device (no CPU fallback)")
+            raise RuntimeError("the ProPainter CUDA engine needs a CUDA device (no CPU fallback)")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self._keep = []
@@ -321,9 +321,10 @@ class Engine:
     # -- workspace sizing
     @staticmethod
     def clip_workspace_bytes(T: int, H: int, W: int) -> int:
-        """Arena size that lets every stage of a T x H x W clip run in its widest batching (measured peaks: 24.3 GB at
-        80 x 640x360, 92 GB at 80 x 1280x720 => ~1.3 kB per frame-pixel; clips beyond ~100 frames are processed in
-        sub-batches of windows / chunks of sub-videos, so the estimate saturates there)."""
+        """Arena size that lets every stage of a T x H x W clip run in its widest batching (~1.4 kB per frame-pixel;
+        clips beyond ~100 frames are processed in sub-batches of windows / chunks of sub-videos, so the estimate
+        saturates there).  reserve_for_clip caps it at 80 % of the device memory; above the cap the stages run smaller
+        batches."""
         return int(1400 * min(T, 100) * H * W + (2 << 30))
 
     def set_workspace_bytes(self, nbytes: int) -> None:

@@ -1,4 +1,4 @@
-"""Inference orchestration with the reference's entry points, executed by the sm_100a engine.
+"""Inference orchestration with the reference's entry points, executed by the sm_90a engine.
 
 Same public names and argument meaning as the reference's ``propainter_inference.py``
 (ProPainterConfig, get_ref_index, compute_flow, complete_flow, image_propagation, feature_propagation,

@@ -1,4 +1,4 @@
-"""ComfyUI nodes "ProPainter Inpainting" / "ProPainter Outpainting" backed by the sm_100a engine.
+"""ComfyUI nodes "ProPainter Inpainting" / "ProPainter Outpainting" backed by the sm_90a engine.
 
 Drop-in for the reference's propainter_nodes.py: same node keys, display names, INPUT_TYPES (names, order,
 defaults, ranges), RETURN_TYPES / RETURN_NAMES, FUNCTION and CATEGORY (reference propainter_nodes.py:38-321).

@@ -1,4 +1,4 @@
-"""Model residency: three checkpoints -> one packed sm_100a engine (reference: utils/model_utils.py:13-59).
+"""Model residency: three checkpoints -> one packed sm_90a engine (reference: utils/model_utils.py:13-59).
 
 ``Models`` keeps the reference's three fields; each is a thin stage handle sharing one ``Engine``.
 Checkpoints are the reference's ``.pth`` state_dict files under ``<package>/weights/``

@@ -1,4 +1,4 @@
-/* C ABI of the B200-native ProPainter inference path (libpropainter_b200.so).
+/* C ABI of the H100-native ProPainter inference path (libpropainter_b200.so).
  *
  * Every entry point takes raw device pointers, sizes and a CUDA stream (as void*, 0 = legacy default
  * stream) and returns 0 on success; on failure pp_last_error() holds a message.  No torch types cross this
@@ -36,7 +36,7 @@ typedef struct PPEngine* pp_handle;
 
 /* Message of the last failing call on this thread. */
 PP_API const char* pp_last_error(void);
-/* Library build id ("propainter_b200 <n> sm_100a"). */
+/* Library build id ("propainter_b200 <n> sm_90a"). */
 PP_API const char* pp_version(void);
 
 /* Create an engine on `device` whose scratch arena is the caller-allocated device buffer
@@ -145,7 +145,7 @@ PP_API int pp_profile_enable(pp_handle h, int on);
 PP_API int pp_profile_dump(pp_handle h, char* buf, size_t cap);
 
 /* ---- single-operator entry points (unit tests and micro-benchmarks) ------------------------------------ */
-/* Generic conv / linear through the tcgen05 implicit-GEMM kernel: x NHWC fp16 [N,H,W,cin_g*groups]. */
+/* Generic conv / linear through the wgmma implicit-GEMM kernel: x NHWC fp16 [N,H,W,cin_g*groups]. */
 PP_API int pp_op_conv(pp_handle h, const char* name, const void* x_f16, int N, int H, int W, int stride, int pad, int dil,
                int replicate, int act, float slope, const void* residual_f16, void* out_f16, void* stream);
 PP_API int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: python -m pytest tests -m gpu).
+"""GPU parity tests (run on an H100: python -m pytest tests -m gpu).
 
 CUDA path (through the C ABI) vs. the golden outputs of the REAL reference / the CPU oracle on identical
 seeded inputs.  Tolerances: the engine stores activations in fp16 and accumulates in fp32, the oracle and the

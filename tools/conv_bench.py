@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 implicit-GEMM conv on representative layers (CUDA events, L2 flushed)."""
+"""Micro-benchmark of the wgmma implicit-GEMM conv on representative layers (CUDA events, L2 flushed)."""
 import math
 import sys
 import os
