@@ -98,10 +98,59 @@ struct Ring {
   uint32_t ph;
 };
 
+// Most filter taps whose [BN x 64] weight tiles share one 16 KB weight stage (HaloParams::tps never exceeds it).
+__host__ __device__ constexpr int halo_max_tps(int bn) { return 128 / bn > 1 ? 128 / bn : 1; }
+
+// One filter tap: 4 k-steps of 16 channels for each m64 block, then the descriptors move on to the next tap.
+template <int BN, int MB>
+__device__ __forceinline__ void halo_tap(float (&acc)[MB][BN / 2], uint64_t (&adesc)[MB], uint64_t& bdesc, uint32_t& accum,
+                                         int& kx, int kw, uint32_t step_x, uint32_t step_row, uint32_t tap16) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int b = 0; b < MB; ++b) ppx::wgmma_f16<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (accum | k) != 0 ? 1u : 0u);
+  accum = 1u;
+  bdesc += tap16;
+  const uint32_t step = ++kx == kw ? step_row : step_x;
+  if (kx == kw) kx = 0;
+#pragma unroll
+  for (int b = 0; b < MB; ++b) adesc[b] += step;
+}
+
+// The wgmmas of one weight stage (tn filter taps) as one commit group.
+// NT > 0 (tn <= NT): the tap count is dispatched to a compile-time constant, so the group is straight-line code.  A
+// runtime-length tap loop puts the group's wgmmas on several control paths; ptxas then injects warpgroup.arrive at the
+// joins (C7519 / C7520) and makes every wgmma wait for the previous one.
+// NT == 0: that runtime loop, for conv_prog_kernel, whose wgmmas ptxas serializes for lack of registers anyway (C7512)
+// and where the unrolled groups only add spills.
+template <int BN, int MB, int NT>
+__device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2], uint64_t (&adesc)[MB], uint64_t bdesc,
+                                               uint32_t& accum, int& kx, int kw, uint32_t step_x, uint32_t step_row,
+                                               uint32_t tap16) {
+  using namespace ppx;
+  if constexpr (NT == 0) {
+    wgmma_fence();
+    for (int tt = 0; tt < tn; ++tt) halo_tap<BN, MB>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+    wgmma_commit();
+  } else {
+    if constexpr (NT > 1) {
+      if (tn < NT) {
+        halo_tap_group<BN, MB, NT - 1>(tn, acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+        return;
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int tt = 0; tt < NT; ++tt) halo_tap<BN, MB>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+    wgmma_commit();
+  }
+}
+
 // Consumer side of one tile, run by each of the two consumer warpgroups: the main loop into register accumulators
 // (MB = h.MT m64 blocks of BN columns), then the epilogue of this warpgroup's pixel rows.  A stage is handed back to
 // its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
-template <int BN, int MB>
+// NT: see halo_tap_group.
+template <int BN, int MB, int NT>
 __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, uint8_t* smem, uint8_t* smem_b, int SA, int SB,
                                           int a_stage_bytes, int b_stage_bytes, uint64_t* a_full, uint64_t* a_empty,
                                           uint64_t* b_full, uint64_t* b_empty, Ring& ra, Ring& rb, float* stg,
@@ -131,22 +180,8 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, uint8_t
     int kx = 0;
     for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
       mbar_wait(&b_full[rb.s], rb.ph);
-      wgmma_fence();
-      uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(smem_b + rb.s * b_stage_bytes));
-      const int tn = min(h.tps, taps - tap0);
-      for (int tt = 0; tt < tn; ++tt) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-#pragma unroll
-          for (int b = 0; b < MB; ++b) wgmma_f16<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (accum | k) != 0 ? 1u : 0u);
-        accum = 1u;
-        bdesc += tap16;
-        const uint32_t step = ++kx == kw ? step_row : step_x;
-        if (kx == kw) kx = 0;
-#pragma unroll
-        for (int b = 0; b < MB; ++b) adesc[b] += step;
-      }
-      wgmma_commit();
+      const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(smem_b + rb.s * b_stage_bytes));
+      halo_tap_group<BN, MB, NT>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
       wgmma_wait<1>();
       if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
       if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
@@ -263,9 +298,10 @@ __global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_
     float* stg = acc_stg + wg * (ppconv::STG_BYTES / 4);
     Ring ra = {0, 0}, rb = {0, 0};
     auto run = [&](auto bn, auto mb) {
+      constexpr int BN = decltype(bn)::value;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
-        halo_tile<decltype(bn)::value, decltype(mb)::value>(h, tile, smem, smem_b, h.SA, h.SB, h.a_stage_bytes, h.b_stage_bytes,
-                                                            a_full, a_empty, b_full, b_empty, ra, rb, stg, stg_out, wg, t128);
+        halo_tile<BN, decltype(mb)::value, halo_max_tps(BN)>(h, tile, smem, smem_b, h.SA, h.SB, h.a_stage_bytes, h.b_stage_bytes,
+                                                             a_full, a_empty, b_full, b_empty, ra, rb, stg, stg_out, wg, t128);
     };
     if constexpr (UPS) ppconv::with_tile_width<128>(p.BN, [&](auto bn) { run(bn, ppconv::IntC<1>{}); });   // MT == 1
     else with_tile_shape(h.MT, p.BN, run);
@@ -523,7 +559,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
         // instances make this kernel spill its accumulators
         ppconv::with_tile_width<128>(h.c.BN, [&](auto bn) {
           for (int tile = blockIdx.x; tile < total_tiles; tile += G)
-            halo_tile<decltype(bn)::value, 1>(h, tile, smem, smem_b, P.SA, P.SB, P.a_stage_bytes, P.b_stage_bytes, a_full,
+            halo_tile<decltype(bn)::value, 1, 0>(h, tile, smem, smem_b, P.SA, P.SB, P.a_stage_bytes, P.b_stage_bytes, a_full,
                                               a_empty, b_full, b_empty, ra, rb, stg, nullptr, wg, t128);
         });
       }
@@ -723,7 +759,7 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
     // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloParams::tps
     static int max_tps = -1;
     if (max_tps < 0) { const char* e = getenv("PP_HALO_TPS"); max_tps = e != nullptr ? atoi(e) : 9; }
-    int tps = 16384 / (bn * 128);
+    int tps = halo_max_tps(bn);
     if (tps > p.kh * p.kw) tps = p.kh * p.kw;
     if (tps > max_tps) tps = max_tps;
     if (tps < 1 || p.ups2x) tps = 1;
