@@ -6,7 +6,6 @@
 #include <vector>
 
 #include "../../include/propainter_b200.h"
-#include "dcn_sample.cuh"
 #include "engine.cuh"
 
 // Makes the engine's device current for the duration of one API call and restores the caller's device afterwards.
@@ -420,28 +419,6 @@ int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* prop_in4_f
   return pp_k_imgprop_step(static_cast<const __half*>(cur4_f16), static_cast<const __half*>(prop_in4_f16),
                            static_cast<__half*>(prop_out4_f16), static_cast<const __half*>(flow_prop_f16),
                            static_cast<const __half*>(flow_check_f16), H, W, as_stream(stream));
-}
-
-int pp_op_dcn_sample(pp_handle h, const void* x_f16, const void* offs_f16, const void* flow_f16, float max_mag,
-                     void* cols_f16, int N, int H, int W, int C, int tiled, void* stream) {
-  PP_HANDLE(h);
-  PP_REQUIRE(x_f16 && offs_f16 && cols_f16, "pp_op_dcn_sample: null pointer");
-  PPDcnArgs a;
-  const __half* x = static_cast<const __half*>(x_f16);
-  // C == 256: cat(x0[128], x1[128]) like the flow-completion alignment; C == 128: one tensor (+ flow) like the generator's
-  a.x0 = x; a.x0_cs = C; a.x0_co = 0; a.C0 = C == 256 ? 128 : C;
-  a.x1 = C == 256 ? x : nullptr; a.x1_cs = C; a.x1_co = 128;
-  a.offs = static_cast<const __half*>(offs_f16); a.offs_cs = 432;
-  a.flow = static_cast<const __half*>(flow_f16); a.flow_cs = 2; a.flow_co = 0;
-  a.max_mag = max_mag; a.cols = static_cast<__half*>(cols_f16); a.C = C; a.N = N; a.H = H; a.W = W;
-  e.launches++;
-  if (tiled) {
-    int handled = 0;
-    PP_TRY(pp_k_dcn_sample_tiled(a, 3, as_stream(stream), &handled));
-    PP_REQUIRE(handled, "pp_op_dcn_sample: the tiled sampler does not handle this shape");
-    return PP_OK;
-  }
-  return pp_k_dcn_sample_plain(a, as_stream(stream));
 }
 
 int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,

@@ -32,12 +32,9 @@ namespace {
 constexpr int NUM_THREADS = 384;   // warpgroup 2: warps 8-9 producers, 10-11 idle (setmaxnreg works per warpgroup)
 constexpr int NUM_EPI_THREADS = 256;   // the two consumer warpgroups
 constexpr int WARP_A = 8, WARP_B = 9;
-// fused x2-upsample variant (UPS): warps 8-11 interpolate the input patch (warp 8 also issues the low-res TMA loads),
-// the weight producer moves to warp 12
-constexpr int UPS_THREADS = 416, UPS_INTERP_THREADS = 128;
-constexpr int UPS_WARP_B = 12;
 constexpr int MAX_SA = 4, MAX_SB = 8;
-// stages; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the barrier block come on top
+// stages and the TMA-store staging tile; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the
+// barrier block come on top (see HaloSmem)
 constexpr int SMEM_BUDGET = 186 * 1024;
 
 struct HaloParams {
@@ -53,10 +50,6 @@ struct HaloParams {
   int flat;          // 1x1 convs: tiles are runs of 128*MT consecutive pixels of the flattened [N*H*W] pixel list
   int n_img;         // images the tile index decomposes over (1 in flat mode)
   int sub_bytes;     // A-view offset between the sub-tiles: 8 pixels (spatial) or 128 pixels (flat)
-  int ups;           // input tensor is half resolution: bilinear x2 (align_corners) on the fly (UPS kernel)
-  int LH, LW;        // low-res source size
-  int LBW, LBH;      // low-res staging box (pixels)
-  int l_stage_bytes;
   int debug;         // bit 0: skip the epilogue math/stores (PP_CONV_NOEPI=1, mainloop-only timing experiments)
   // flat-mode layers with few K chunks are bound by the epilogue's per-thread 32-byte global stores (one L1 wavefront per
   // lane).  tstore: the epilogue writes the fp16 tile into a 128B-swizzled shared-memory staging tile and ONE thread
@@ -92,11 +85,55 @@ __device__ __forceinline__ TileCoord decode_tile(const HaloParams& h, int tile) 
   return t;
 }
 
-// position in a shared-memory ring of stages (consumer side)
+__host__ __device__ inline int halo_total_tiles(const HaloParams& h) {
+  return h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * h.c.groups;   // < 2^31, checked by halo_configure
+}
+
+// position in a shared-memory ring of stages
 struct Ring {
   int s;
   uint32_t ph;
 };
+
+// Shared-memory carve-up of both halo kernels, from the 1024-byte aligned base:
+//   SA patch stages | SB weight stages | barrier block (1 KB) | TMA-store staging (out_bytes) | 2 accumulator staging tiles
+// The launchers call it with base == nullptr and read only `bytes`.
+struct HaloSmem {
+  uint8_t* a;                  // patch stages (TMA, 128B swizzle: 1024-byte aligned)
+  uint8_t* b;                  // weight stages
+  int SA, SB, a_stage_bytes, b_stage_bytes;
+  uint64_t *a_full, *a_empty, *b_full, *b_empty;
+  uint64_t* spare;             // one more barrier (conv_prog_kernel: layer_go)
+  uint8_t* out_stg;            // TMA-store staging tiles, 1024-byte aligned; nullptr without them
+  float* acc_stg;              // ppconv::STG_BYTES per consumer warpgroup
+  int bytes;                   // dynamic shared memory, including the slack that aligns the base
+};
+
+__host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage_bytes, int SB, int b_stage_bytes,
+                                              int out_bytes) {
+  const int b_off = SA * a_stage_bytes, bar_off = b_off + SB * b_stage_bytes, out_off = bar_off + 1024;
+  const int acc_off = out_off + out_bytes;
+  HaloSmem m;
+  m.SA = SA; m.SB = SB; m.a_stage_bytes = a_stage_bytes; m.b_stage_bytes = b_stage_bytes;
+  m.a = base;
+  m.b = base + b_off;
+  m.a_full = reinterpret_cast<uint64_t*>(base + bar_off);
+  m.a_empty = m.a_full + MAX_SA;
+  m.b_full = m.a_empty + MAX_SA;
+  m.b_empty = m.b_full + MAX_SB;
+  m.spare = m.b_empty + MAX_SB;
+  m.out_stg = out_bytes > 0 ? base + out_off : nullptr;   // a constant in conv_prog_kernel: one live pointer less
+  m.acc_stg = reinterpret_cast<float*>(base + acc_off);
+  m.bytes = 1024 + acc_off + 2 * ppconv::STG_BYTES;
+  return m;
+}
+
+// The 1024-byte aligned base of the dynamic shared memory.
+__device__ __forceinline__ uint8_t* halo_smem_base() {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = ppx::smem_u32(smem_raw);
+  return smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+}
 
 // Most filter taps whose [BN x 64] weight tiles share one 16 KB weight stage (HaloParams::tps never exceeds it).
 __host__ __device__ constexpr int halo_max_tps(int bn) { return 128 / bn > 1 ? 128 / bn : 1; }
@@ -151,10 +188,8 @@ __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2],
 // its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
 // NT: see halo_tap_group.
 template <int BN, int MB, int NT>
-__device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, uint8_t* smem, uint8_t* smem_b, int SA, int SB,
-                                          int a_stage_bytes, int b_stage_bytes, uint64_t* a_full, uint64_t* a_empty,
-                                          uint64_t* b_full, uint64_t* b_empty, Ring& ra, Ring& rb, float* stg,
-                                          uint8_t* stg_out, int wg, int t128) {
+__device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
+                                          int wg, int t128) {
   using namespace ppx;
   const PPConvParams& p = h.c;
   const int taps = p.kh * p.kw;
@@ -173,35 +208,35 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, uint8_t
   uint32_t accum = 0;
   int pend_a = -1, pend_b = -1;
   for (int c = 0; c < h.chunks; ++c) {
-    mbar_wait(&a_full[ra.s], ra.ph);
+    mbar_wait(&m.a_full[ra.s], ra.ph);
     uint64_t adesc[MB];
 #pragma unroll
-    for (int b = 0; b < MB; ++b) adesc[b] = gmma_desc_sw128_kmajor(smem_u32(smem + ra.s * a_stage_bytes) + aoff[b], sbo);
+    for (int b = 0; b < MB; ++b) adesc[b] = gmma_desc_sw128_kmajor(smem_u32(m.a + ra.s * m.a_stage_bytes) + aoff[b], sbo);
     int kx = 0;
     for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
-      mbar_wait(&b_full[rb.s], rb.ph);
-      const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(smem_b + rb.s * b_stage_bytes));
+      mbar_wait(&m.b_full[rb.s], rb.ph);
+      const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(m.b + rb.s * m.b_stage_bytes));
       halo_tap_group<BN, MB, NT>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
       wgmma_wait<1>();
-      if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
-      if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+      if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
+      if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
       pend_b = rb.s;
       pend_a = tap0 + h.tps >= taps ? ra.s : -1;
-      if (++rb.s == SB) { rb.s = 0; rb.ph ^= 1; }
+      if (++rb.s == m.SB) { rb.s = 0; rb.ph ^= 1; }
     }
-    if (++ra.s == SA) { ra.s = 0; ra.ph ^= 1; }
+    if (++ra.s == m.SA) { ra.s = 0; ra.ph ^= 1; }
   }
   wgmma_wait<0>();
 #pragma unroll
   for (int b = 0; b < MB; ++b) wgmma_fence_acc(acc[b]);
-  if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
-  if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+  if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
+  if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
 
   // ---- epilogue.  TMA-store path: staging tile of the sub-tile, its barrier (one warpgroup when MT == 2, both else)
   const bool skip = (h.debug & 1) != 0;
   const int bar_id = 2 + (MB == 2 ? wg : 0), bar_n = MB == 2 ? 128 : 256;
   const bool issuer = t128 == 0 && (MB == 2 || wg == 0);
-  uint8_t* so = h.tstore ? stg_out + (MB == 2 ? wg : 0) * h.out_stage_bytes : nullptr;
+  uint8_t* so = h.tstore ? m.out_stg + (MB == 2 ? wg : 0) * h.out_stage_bytes : nullptr;
   if (so != nullptr) {
     if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
     named_bar(bar_id, bar_n);
@@ -253,197 +288,102 @@ __device__ __forceinline__ void with_tile_shape(int mt, int bn, F&& f) {
   else ppconv::with_tile_width<256>(bn, [&](auto n) { f(n, ppconv::IntC<1>{}); });
 }
 
-template <bool UPS>
-__global__ void __launch_bounds__(UPS ? UPS_THREADS : NUM_THREADS, 1) conv_halo_kernel(const __grid_constant__ HaloParams h) {
+// Thread 0: the barriers of both rings (full: the producer's arrival + transaction bytes, empty: every consumer thread).
+__device__ __forceinline__ void halo_smem_init_barriers(const HaloSmem& m) {
+  using namespace ppx;
+  for (int s = 0; s < m.SA; ++s) { mbar_init(&m.a_full[s], 1); mbar_init(&m.a_empty[s], NUM_EPI_THREADS); }
+  for (int s = 0; s < m.SB; ++s) { mbar_init(&m.b_full[s], 1); mbar_init(&m.b_empty[s], NUM_EPI_THREADS); }
+  mbar_fence_init();
+}
+
+// Input patch producer (TMA, one elected thread): one box load per 64-channel chunk of each of this CTA's tiles of one
+// layer.  `r` runs on across the layers of a program.
+__device__ __forceinline__ void halo_produce_patches(const HaloParams& h, const HaloSmem& m, Ring& r) {
   using namespace ppx;
   const PPConvParams& p = h.c;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* smem_b = smem + h.SA * h.a_stage_bytes;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem_b + h.SB * h.b_stage_bytes);
-  uint64_t* a_empty = a_full + MAX_SA;
-  uint64_t* b_full = a_empty + MAX_SA;
-  uint64_t* b_empty = b_full + MAX_SB;
-  uint64_t* l_full = b_empty + MAX_SB;     // UPS: low-res staging ring (2 stages)
-  uint64_t* l_empty = l_full + 2;
-  uint8_t* stg_out = smem_b + h.SB * h.b_stage_bytes + 2048;     // TMA-store staging (flat layers), 1024-byte aligned
-  float* acc_stg = reinterpret_cast<float*>(smem_b + h.SB * h.b_stage_bytes + 1024 + (UPS ? 2 * h.l_stage_bytes : 0) +
-                                            (h.tstore ? 1024 + h.MT * h.out_stage_bytes : 0));
-  constexpr int W_B = UPS ? UPS_WARP_B : WARP_B;
-
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * p.groups;
-  const int taps = p.kh * p.kw;
-
-  if (tid == 0) {
-    for (int s = 0; s < h.SA; ++s) { mbar_init(&a_full[s], UPS ? UPS_INTERP_THREADS : 1); mbar_init(&a_empty[s], NUM_EPI_THREADS); }
-    if (UPS) for (int s = 0; s < 2; ++s) { mbar_init(&l_full[s], 1); mbar_init(&l_empty[s], UPS_INTERP_THREADS); }
-    for (int s = 0; s < h.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], NUM_EPI_THREADS); }
-    mbar_fence_init();
+  const int total_tiles = halo_total_tiles(h);
+  const uint32_t bytes = (uint32_t)(h.BW * h.BH * 128);
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const TileCoord t = decode_tile(h, tile);
+    const int x0 = h.flat ? t.tx * (128 * h.MT) : t.tx * (8 * h.MT) - p.pw, y0 = h.flat ? 0 : t.ty * 16 - p.ph;
+    for (int c = 0; c < h.chunks; ++c) {
+      const int ci = c * 64;
+      int q = 0;
+#pragma unroll
+      for (int k = 1; k < 4; ++k)
+        if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
+      const int ch0 = t.g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
+      mbar_wait(&m.a_empty[r.s], r.ph ^ 1);
+      mbar_arrive_expect_tx(&m.a_full[r.s], bytes);
+      tma_load_4d(smem_u32(m.a + r.s * m.a_stage_bytes), &h.tmap[q], ch0, x0, y0, t.img, &m.a_full[r.s]);
+      if (++r.s == m.SA) { r.s = 0; r.ph ^= 1; }
+    }
   }
+}
+
+// Weight tile producer (bulk copy, one elected thread): per chunk, the [BN x 64] tiles of the filter taps in groups of
+// h.tps per stage.  `r` runs on across the layers of a program.
+__device__ __forceinline__ void halo_produce_weights(const HaloParams& h, const HaloSmem& m, Ring& r) {
+  using namespace ppx;
+  const PPConvParams& p = h.c;
+  const int total_tiles = halo_total_tiles(h);
+  const int taps = p.kh * p.kw;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const TileCoord t = decode_tile(h, tile);
+    const int n0 = t.n_idx * p.BN;
+    const uint32_t bytes = (uint32_t)(min(p.BN, p.Cout_g_pad - n0) * 128);
+    const __half* wbase = p.wpacked + ((long long)t.g * p.num_kc * p.Cout_g_pad + n0) * 64;
+    for (int c = 0; c < h.chunks; ++c) {
+      for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
+        const int tn = min(h.tps, taps - tap0);
+        mbar_wait(&m.b_empty[r.s], r.ph ^ 1);
+        mbar_arrive_expect_tx(&m.b_full[r.s], bytes * (uint32_t)tn);
+        for (int t = 0; t < tn; ++t) {
+          const int kc = (tap0 + t) * h.chunks + c;
+          bulk_g2s(smem_u32(m.b + r.s * m.b_stage_bytes + t * p.BN * 128), wbase + (long long)kc * p.Cout_g_pad * 64, bytes,
+                   &m.b_full[r.s]);
+        }
+        if (++r.s == m.SB) { r.s = 0; r.ph ^= 1; }
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_kernel(const __grid_constant__ HaloParams h) {
+  using namespace ppx;
+  const HaloSmem m =
+      halo_smem(halo_smem_base(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, h.tstore ? h.MT * h.out_stage_bytes : 0);
+  const int tid = threadIdx.x, warp = tid >> 5;
+  if (tid == 0) halo_smem_init_barriers(m);
   __syncthreads();
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   // 168 registers per thread at launch; the producer warpgroup gives its registers to the accumulator holders (an
   // increase can only use what this CTA released: 2 x 128 x (232 - 168) == 128 x (168 - 40))
-  if constexpr (!UPS) {
-    if (warp < 8) setmaxnreg_inc<232>();
-    else setmaxnreg_dec<40>();
-  }
+  if (warp < 8) setmaxnreg_inc<232>();
+  else setmaxnreg_dec<40>();
   if (warp < 8) {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue
     const int wg = tid >> 7, t128 = tid & 127;
-    float* stg = acc_stg + wg * (ppconv::STG_BYTES / 4);
+    float* stg = m.acc_stg + wg * (ppconv::STG_BYTES / 4);
     Ring ra = {0, 0}, rb = {0, 0};
-    auto run = [&](auto bn, auto mb) {
+    const int total_tiles = halo_total_tiles(h);
+    with_tile_shape(h.MT, h.c.BN, [&](auto bn, auto mb) {
       constexpr int BN = decltype(bn)::value;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
-        halo_tile<BN, decltype(mb)::value, halo_max_tps(BN)>(h, tile, smem, smem_b, h.SA, h.SB, h.a_stage_bytes, h.b_stage_bytes,
-                                                             a_full, a_empty, b_full, b_empty, ra, rb, stg, stg_out, wg, t128);
-    };
-    if constexpr (UPS) ppconv::with_tile_width<128>(p.BN, [&](auto bn) { run(bn, ppconv::IntC<1>{}); });   // MT == 1
-    else with_tile_shape(h.MT, p.BN, run);
+        halo_tile<BN, decltype(mb)::value, halo_max_tps(BN)>(h, tile, m, ra, rb, stg, wg, t128);
+    });
     if (h.tstore) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // outstanding stores of this thread complete
-  } else if (UPS && warp < 12) {
-    // ------------------------------------------------------------------ fused bilinear x2 (align_corners=True) producer
-    // The conv's input is the x2 upsampling of a half-resolution tensor (reference deconv = F.interpolate + conv).
-    // Per 64-channel chunk the elected lane of warp 8 TMA-loads the low-res patch that covers the 18x18 hi-res patch
-    // into a 2-stage staging ring; the 128 threads interpolate it (fp32, one rounding, same expression as the
-    // stand-alone upsample kernel) straight into the 128B-swizzled A stage.  Hi-res pixels outside the image are the
-    // conv's zero padding.  The upsampled tensor (4x the pixels) never exists in memory.
-    const int it_id = tid - 256;
-    uint8_t* stg = smem_b + h.SB * h.b_stage_bytes + 1024;     // staging ring behind the barrier block
-    const float sy = (float)(h.LH - 1) / (float)(2 * h.LH - 1), sx = (float)(h.LW - 1) / (float)(2 * h.LW - 1);
-    const uint32_t lbytes = (uint32_t)(h.LBW * h.LBH * 128);
-    const bool issuer = warp == 8 && elect_one();
-    auto low_origin = [&](const TileCoord& t, int& xlo, int& ylo) {
-      const int X0 = t.tx * (8 * h.MT) - p.pw, Y0 = t.ty * 16 - p.ph;
-      xlo = (int)(sx * (float)max(X0, 0));
-      ylo = (int)(sy * (float)max(Y0, 0));
-    };
-    auto issue = [&](int tile, int c, int ls, uint32_t lph) {
-      const TileCoord t = decode_tile(h, tile);
-      int xlo, ylo;
-      low_origin(t, xlo, ylo);
-      mbar_wait(&l_empty[ls], lph ^ 1);
-      mbar_arrive_expect_tx(&l_full[ls], lbytes);
-      tma_load_4d(smem_u32(stg + ls * h.l_stage_bytes), &h.tmap[0], c * 64, xlo, ylo, t.img, &l_full[ls]);
-    };
-    int ls = 0, sa = 0;
-    uint32_t lph = 0, pa = 0;
-    // producer-side schedule of staging slots: (stage, phase) advance once per issued chunk
-    int is_ls = 0;
-    uint32_t is_ph = 0;
-    if (issuer && blockIdx.x < total_tiles) {
-      issue(blockIdx.x, 0, is_ls, is_ph);
-      if (++is_ls == 2) { is_ls = 0; is_ph ^= 1; }
+  } else if (warp == WARP_A) {
+    if (elect_one()) {
+      Ring r = {0, 0};
+      halo_produce_patches(h, m, r);
     }
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const TileCoord t = decode_tile(h, tile);
-      const int X0 = t.tx * (8 * h.MT) - p.pw, Y0 = t.ty * 16 - p.ph;
-      int xlo, ylo;
-      low_origin(t, xlo, ylo);
-      for (int c = 0; c < h.chunks; ++c) {
-        if (issuer) {   // prefetch the next chunk's low-res patch
-          int nt = tile, nc = c + 1;
-          if (nc == h.chunks) { nc = 0; nt += gridDim.x; }
-          if (nt < total_tiles) {
-            issue(nt, nc, is_ls, is_ph);
-            if (++is_ls == 2) { is_ls = 0; is_ph ^= 1; }
-          }
-        }
-        __syncwarp();
-        mbar_wait(&l_full[ls], lph);
-        mbar_wait(&a_empty[sa], pa ^ 1);
-        const uint8_t* src = stg + ls * h.l_stage_bytes;
-        uint8_t* dstA = smem + sa * h.a_stage_bytes;
-        const int items = h.BW * h.BH * 8;
-        for (int item = it_id; item < items; item += UPS_INTERP_THREADS) {
-          const int ch = item & 7, pp = item >> 3;
-          const int py = pp / h.BW, px = pp - py * h.BW;
-          const int Y = Y0 + py, X = X0 + px;
-          uint4 o = make_uint4(0, 0, 0, 0);
-          if ((unsigned)Y < (unsigned)(2 * h.LH) && (unsigned)X < (unsigned)(2 * h.LW)) {
-            const float fy = sy * (float)Y, fx = sx * (float)X;
-            const int y0 = (int)fy, x0 = (int)fx;
-            const int y1 = min(y0 + 1, h.LH - 1), x1 = min(x0 + 1, h.LW - 1);
-            const float ly = fy - (float)y0, lx = fx - (float)x0;
-            const float w00 = (1.f - ly) * (1.f - lx), w01 = (1.f - ly) * lx, w10 = ly * (1.f - lx), w11 = ly * lx;
-            const uint8_t* r0 = src + ((y0 - ylo) * h.LBW - xlo) * 128 + ch * 16;
-            const uint8_t* r1 = src + ((y1 - ylo) * h.LBW - xlo) * 128 + ch * 16;
-            const uint4 qa = *reinterpret_cast<const uint4*>(r0 + x0 * 128), qb = *reinterpret_cast<const uint4*>(r0 + x1 * 128);
-            const uint4 qc = *reinterpret_cast<const uint4*>(r1 + x0 * 128), qd = *reinterpret_cast<const uint4*>(r1 + x1 * 128);
-            const __half2* ah = reinterpret_cast<const __half2*>(&qa);
-            const __half2* bh = reinterpret_cast<const __half2*>(&qb);
-            const __half2* chh = reinterpret_cast<const __half2*>(&qc);
-            const __half2* dh = reinterpret_cast<const __half2*>(&qd);
-            __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 fa = __half22float2(ah[i]), fb = __half22float2(bh[i]), fc = __half22float2(chh[i]),
-                           fd = __half22float2(dh[i]);
-              oh[i] = __floats2half2_rn(w00 * fa.x + w01 * fb.x + w10 * fc.x + w11 * fd.x,
-                                        w00 * fa.y + w01 * fb.y + w10 * fc.y + w11 * fd.y);
-            }
-          }
-          *reinterpret_cast<uint4*>(dstA + pp * 128 + ((ch ^ (pp & 7)) << 4)) = o;
-        }
-        fence_proxy_async();            // generic-proxy writes of the A stage -> visible to wgmma
-        mbar_arrive(&a_full[sa]);
-        mbar_arrive(&l_empty[ls]);
-        if (++ls == 2) { ls = 0; lph ^= 1; }
-        if (++sa == h.SA) { sa = 0; pa ^= 1; }
-      }
-    }
-  } else if (!UPS && warp == WARP_A) {
-    // ------------------------------------------------------------------ input patch producer (TMA)
-    if (ppx::elect_one()) {
-      int s = 0;
-      uint32_t phase = 0;
-      const uint32_t bytes = (uint32_t)(h.BW * h.BH * 128);
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const TileCoord t = decode_tile(h, tile);
-        const int x0 = h.flat ? t.tx * (128 * h.MT) : t.tx * (8 * h.MT) - p.pw, y0 = h.flat ? 0 : t.ty * 16 - p.ph;
-        for (int c = 0; c < h.chunks; ++c) {
-          const int ci = c * 64;
-          int q = 0;
-#pragma unroll
-          for (int k = 1; k < 4; ++k)
-            if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
-          const int ch0 = t.g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
-          mbar_wait(&a_empty[s], phase ^ 1);
-          mbar_arrive_expect_tx(&a_full[s], bytes);
-          tma_load_4d(smem_u32(smem + s * h.a_stage_bytes), &h.tmap[q], ch0, x0, y0, t.img, &a_full[s]);
-          if (++s == h.SA) { s = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == W_B) {
-    // ------------------------------------------------------------------ weight tile producer (bulk copy)
-    if (ppx::elect_one()) {
-      int s = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const TileCoord t = decode_tile(h, tile);
-        const int n0 = t.n_idx * p.BN;
-        const uint32_t bytes = (uint32_t)(min(p.BN, p.Cout_g_pad - n0) * 128);
-        const __half* wbase = p.wpacked + ((long long)t.g * p.num_kc * p.Cout_g_pad + n0) * 64;
-        for (int c = 0; c < h.chunks; ++c) {
-          for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
-            const int tn = min(h.tps, taps - tap0);
-            mbar_wait(&b_empty[s], phase ^ 1);
-            mbar_arrive_expect_tx(&b_full[s], bytes * (uint32_t)tn);
-            for (int t = 0; t < tn; ++t) {
-              const int kc = (tap0 + t) * h.chunks + c;
-              bulk_g2s(smem_u32(smem_b + s * h.b_stage_bytes + t * p.BN * 128), wbase + (long long)kc * p.Cout_g_pad * 64, bytes,
-                       &b_full[s]);
-            }
-            if (++s == h.SB) { s = 0; phase ^= 1; }
-          }
-        }
-      }
+  } else if (warp == WARP_B) {
+    if (elect_one()) {
+      Ring r = {0, 0};
+      halo_produce_weights(h, m, r);
     }
   }
 }
@@ -495,24 +435,14 @@ __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_constant__ ProgParams P) {
   using namespace ppx;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* smem_b = smem + P.SA * P.a_stage_bytes;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem_b + P.SB * P.b_stage_bytes);
-  uint64_t* a_empty = a_full + MAX_SA;
-  uint64_t* b_full = a_empty + MAX_SA;
-  uint64_t* b_empty = b_full + MAX_SB;
-  uint64_t* layer_go = b_empty + MAX_SB;   // the CTA's one poller (TMA producer thread) -> consumers: layer li may start
-  float* acc_stg = reinterpret_cast<float*>(smem_b + P.SB * P.b_stage_bytes + 1024);
+  const HaloSmem m = halo_smem(halo_smem_base(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes, 0);
+  uint64_t* layer_go = m.spare;   // the CTA's one poller (TMA producer thread) -> consumers: layer li may start
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const unsigned int G = gridDim.x;
   if (tid == 0) {
     mbar_init(layer_go, 1);
-    for (int s = 0; s < P.SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], NUM_EPI_THREADS); }
-    for (int s = 0; s < P.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], NUM_EPI_THREADS); }
-    mbar_fence_init();
+    halo_smem_init_barriers(m);
   }
   __syncthreads();
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -523,7 +453,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
   if (warp < 8) {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue (+ the sampling layers)
     const int wg = tid >> 7, t128 = tid & 127;
-    float* stg = acc_stg + wg * (ppconv::STG_BYTES / 4);
+    float* stg = m.acc_stg + wg * (ppconv::STG_BYTES / 4);
     Ring ra = {0, 0}, rb = {0, 0};
     for (int li = 0; li < P.n_layers; ++li) {
       // inputs of this layer (residuals, sampling sources) were written by the previous one: the producer thread polls
@@ -554,13 +484,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
         }
       } else {
         const HaloParams& h = P.layer[li];
-        const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * h.c.groups;
+        const int total_tiles = halo_total_tiles(h);
         // program layers are configured with MT == 1 and BN <= 128 (halo_configure, one_wave): wider or two-sub-tile
         // instances make this kernel spill its accumulators
         ppconv::with_tile_width<128>(h.c.BN, [&](auto bn) {
           for (int tile = blockIdx.x; tile < total_tiles; tile += G)
-            halo_tile<decltype(bn)::value, 1, 0>(h, tile, smem, smem_b, P.SA, P.SB, P.a_stage_bytes, P.b_stage_bytes, a_full,
-                                              a_empty, b_full, b_empty, ra, rb, stg, nullptr, wg, t128);
+            halo_tile<decltype(bn)::value, 1, 0>(h, tile, m, ra, rb, stg, wg, t128);
         });
       }
       // publish this CTA's part of the layer: stores -> async proxy, CTA-wide meet of the writers, one arrival
@@ -578,69 +507,23 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
     }
   } else if (warp == WARP_A) {
     // ------------------------------------------------------------------ input patch producer (TMA)
-    if (ppx::elect_one()) {
-      int s = 0;
-      uint32_t phase = 0;
+    if (elect_one()) {
+      Ring r = {0, 0};
       for (int li = 0; li < P.n_layers; ++li) {
         if (li > 0) {     // the CTA's only poller: every CTA finished layer li-1
           prog_wait(P.counter, P.base + (unsigned int)li * G);
           fence_proxy_async_global();
         }
         mbar_arrive(layer_go);
-        if (P.kind[li] != PROG_CONV) continue;
-        const HaloParams& h = P.layer[li];
-        const PPConvParams& p = h.c;
-        const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * p.groups;
-        const uint32_t bytes = (uint32_t)(h.BW * h.BH * 128);
-        for (int tile = blockIdx.x; tile < total_tiles; tile += G) {
-          const TileCoord t = decode_tile(h, tile);
-          const int x0 = h.flat ? t.tx * (128 * h.MT) : t.tx * (8 * h.MT) - p.pw, y0 = h.flat ? 0 : t.ty * 16 - p.ph;
-          for (int c = 0; c < h.chunks; ++c) {
-            const int ci = c * 64;
-            int q = 0;
-#pragma unroll
-            for (int k = 1; k < 4; ++k)
-              if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
-            const int ch0 = t.g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
-            mbar_wait(&a_empty[s], phase ^ 1);
-            mbar_arrive_expect_tx(&a_full[s], bytes);
-            tma_load_4d(smem_u32(smem + s * P.a_stage_bytes), &h.tmap[q], ch0, x0, y0, t.img, &a_full[s]);
-            if (++s == P.SA) { s = 0; phase ^= 1; }
-          }
-        }
+        if (P.kind[li] == PROG_CONV) halo_produce_patches(P.layer[li], m, r);
       }
     }
   } else if (warp == WARP_B) {
     // ------------------------------------------------------------------ weight tile producer: never waits for a layer
-    if (ppx::elect_one()) {
-      int s = 0;
-      uint32_t phase = 0;
-      for (int li = 0; li < P.n_layers; ++li) {
-        if (P.kind[li] != PROG_CONV) continue;
-        const HaloParams& h = P.layer[li];
-        const PPConvParams& p = h.c;
-        const int total_tiles = h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * p.groups;
-        const int taps = p.kh * p.kw;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += G) {
-          const TileCoord t = decode_tile(h, tile);
-          const int n0 = t.n_idx * p.BN;
-          const uint32_t bytes = (uint32_t)(min(p.BN, p.Cout_g_pad - n0) * 128);
-          const __half* wbase = p.wpacked + ((long long)t.g * p.num_kc * p.Cout_g_pad + n0) * 64;
-          for (int c = 0; c < h.chunks; ++c) {
-            for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
-              const int tn = min(h.tps, taps - tap0);
-              mbar_wait(&b_empty[s], phase ^ 1);
-              mbar_arrive_expect_tx(&b_full[s], bytes * (uint32_t)tn);
-              for (int t = 0; t < tn; ++t) {
-                const int kc = (tap0 + t) * h.chunks + c;
-                bulk_g2s(smem_u32(smem_b + s * P.b_stage_bytes + t * p.BN * 128), wbase + (long long)kc * p.Cout_g_pad * 64, bytes,
-                         &b_full[s]);
-              }
-              if (++s == P.SB) { s = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
+    if (elect_one()) {
+      Ring r = {0, 0};
+      for (int li = 0; li < P.n_layers; ++li)
+        if (P.kind[li] == PROG_CONV) halo_produce_weights(P.layer[li], m, r);
     }
   }
 }
@@ -667,19 +550,17 @@ EncodeTiledFn encode_fn() {
 
 // 0 = not eligible (caller falls back to the cp.async implicit-GEMM kernel), 1 = eligible.
 int pp_conv_halo_eligible(const PPConvParams& p) {
-  static int enabled = -1, allow_1x1 = -1;
+  static int enabled = -1;
   if (enabled < 0) {
     const char* e = getenv("PP_CONV_HALO");
     enabled = (e == nullptr || atoi(e) != 0) ? 1 : 0;
-    e = getenv("PP_HALO_1X1");
-    allow_1x1 = (e == nullptr || atoi(e) != 0) ? 1 : 0;
   }
   if (!enabled) return 0;
   if (p.sh != 1 || p.sw != 1 || p.pad_replicate) return 0;
   const bool flat = p.kh * p.kw == 1;
   if (flat) {
     // 1x1 conv / linear layer: tiles are runs of consecutive pixels; a ragged channel tail is zero-filled by TMA
-    if (!allow_1x1 || p.ph != 0 || p.pw != 0 || p.groups != 1) return 0;
+    if (p.ph != 0 || p.pw != 0 || p.groups != 1) return 0;
   } else if (p.Cin % 64 != 0) {
     return 0;   // packed K order is (tap, ci): 64-channel chunks must not straddle taps
   }
@@ -689,7 +570,6 @@ int pp_conv_halo_eligible(const PPConvParams& p) {
   }
   if ((p.kw - 1) * p.dw + 16 > 256 || (p.kh - 1) * p.dh + 16 > 256) return 0;
   if ((long long)p.N * p.OH * p.OW < 128) return 0;
-  if (p.ups2x && (flat || p.nseg != 1 || p.groups != 1 || p.H % 2 != 0 || p.W % 2 != 0 || p.H < 4 || p.W < 4)) return 0;
   return encode_fn() != nullptr ? 1 : 0;
 }
 
@@ -701,11 +581,42 @@ int halo_num_sms(int* out) {
     int dev = 0;
     PP_CUDA_CHECK(cudaGetDevice(&dev));
     PP_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_prog_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
   }
   *out = num_sms;
+  return PP_OK;
+}
+
+// Pipeline depth for stages of a_bytes / b_bytes in `budget` bytes: the deepest patch ring (3 or 2 stages) that leaves
+// room for at least 3 weight stages, and as many weight stages as fit (at most MAX_SB).  false: nothing fits.
+bool halo_stages(int budget, int a_bytes, int b_bytes, int& sa, int& sb) {
+  for (sa = 3; sa >= 2; --sa) {
+    sb = (budget - sa * a_bytes) / b_bytes;
+    if (sb >= 3) {
+      if (sb > MAX_SB) sb = MAX_SB;
+      return true;
+    }
+  }
+  return false;
+}
+
+// One CTA of NUM_THREADS per SM, with programmatic dependent launch (the kernels' griddepcontrol.wait orders the data).
+template <class Params>
+int halo_launch(void (*kernel)(Params), const Params& params, int grid, int smem_bytes, cudaStream_t stream) {
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = smem_bytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, params));
+  PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
 
@@ -727,19 +638,15 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   auto count = [&](int mt, int bn_) {
     return (long long)pp_ceil_div(p.Cout_g_pad, bn_) * tiles_x(mt) * tiles_y * n_img * p.groups;
   };
-  // fused-upsample layers run 416 threads (at most 157 registers each): one sub-tile per CTA keeps the accumulators small
-  int mt = 2;
-  if (p.ups2x || count(2, bn) < num_sms) mt = 1;
+  int mt = count(2, bn) < num_sms ? 1 : 2;
   while (count(mt, bn) < num_sms && bn >= 64 && bn % 32 == 0) bn /= 2;   // small launches: more, narrower tiles
-  if (one_wave && !p.ups2x) {
+  if (one_wave) {
     // largest tile count that still fits one wave: 128-pixel tiles, N split into 1..8 tiles of <= 128 columns (the
     // only shapes the program kernel instantiates; the fallback bn above is <= 128 too)
     mt = 1;
-    static int min_bn = -1;
-    if (min_bn < 0) { const char* e = getenv("PP_PROG_MIN_BN"); min_bn = e != nullptr ? atoi(e) : 16; }
     for (int nt = 8; nt >= 1; --nt) {
       const int b = pp_ceil_div(pp_ceil_div(p.Cout_g_pad, nt), 16) * 16;
-      if (b > 128 || b < 16 || (b < min_bn && nt > 1)) continue;
+      if (b > 128 || b < 16) continue;
       if (count(1, b) <= num_sms) { mt = 1; bn = b; break; }
     }
   }
@@ -755,52 +662,27 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   h.n_tiles = pp_ceil_div(p.Cout_g_pad, bn);
   h.chunks = pp_ceil_div(p.Cin, 64);
   h.a_stage_bytes = pp_ceil_div(h.BW * h.BH * 128, 1024) * 1024;
-  {
-    // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloParams::tps
-    static int max_tps = -1;
-    if (max_tps < 0) { const char* e = getenv("PP_HALO_TPS"); max_tps = e != nullptr ? atoi(e) : 9; }
-    int tps = halo_max_tps(bn);
-    if (tps > p.kh * p.kw) tps = p.kh * p.kw;
-    if (tps > max_tps) tps = max_tps;
-    if (tps < 1 || p.ups2x) tps = 1;
-    h.tps = tps;
-  }
+  // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloParams::tps
+  h.tps = min(halo_max_tps(bn), p.kh * p.kw);
   h.b_stage_bytes = h.tps * bn * 128;
-  h.ups = p.ups2x ? 1 : 0;
-  h.LH = p.H / 2; h.LW = p.W / 2;
-  h.LBW = (h.BW - 1) / 2 + 3; h.LBH = (h.BH - 1) / 2 + 3;      // low-res pixels that can feed BW x BH hi-res ones
-  h.l_stage_bytes = h.ups ? pp_ceil_div(h.LBW * h.LBH * 128, 1024) * 1024 : 0;
   // TMA-store epilogue (see HaloParams::tstore): flat layers with few K chunks, plain fp16 output
   h.tstore = 0;
   h.out_stage_bytes = 0;
-  {
-    static int ts_on = -1;
-    if (ts_on < 0) { const char* e = getenv("PP_TMA_STORE"); ts_on = (e == nullptr || atoi(e) != 0) ? 1 : 0; }
-    if (ts_on && !one_wave && flat && !h.ups && p.epi == PP_EPI_STD && !p.out_fp32 && p.groups == 1 && p.out_gstep == 0 &&
-        bn % 64 == 0 && p.vec_ok && h.chunks <= 16 && p.out_cstride % 8 == 0 && p.out_coff % 8 == 0 &&
-        (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
-      h.tstore = 1;
-      h.out_stage_bytes = (bn / 64) * 16384;
-    }
+  if (!one_wave && flat && p.epi == PP_EPI_STD && !p.out_fp32 && p.groups == 1 && p.out_gstep == 0 && bn % 64 == 0 &&
+      p.vec_ok && h.chunks <= 16 && p.out_cstride % 8 == 0 && p.out_coff % 8 == 0 &&
+      (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
+    h.tstore = 1;
+    h.out_stage_bytes = (bn / 64) * 16384;
   }
-  const int budget = SMEM_BUDGET - 2 * h.l_stage_bytes - (h.ups ? 1024 : 0) - (h.tstore ? mt * h.out_stage_bytes + 1024 : 0);
-  int sa = h.ups ? 2 : 3, sb = 0;
-  for (; sa >= 2; --sa) {
-    sb = (budget - sa * h.a_stage_bytes) / h.b_stage_bytes;
-    if (sb >= 3) break;
-  }
-  if (h.tstore && !(sa >= 2 && sb >= 3)) {      // no room for the staging tile: plain epilogue
-    h.tstore = 0;
+  int sa = 0, sb = 0;
+  if (h.tstore && !halo_stages(SMEM_BUDGET - mt * h.out_stage_bytes, h.a_stage_bytes, h.b_stage_bytes, sa, sb)) {
+    h.tstore = 0;                                 // no room for the staging tile: plain epilogue
     h.out_stage_bytes = 0;
-    const int budget2 = SMEM_BUDGET - 2 * h.l_stage_bytes - (h.ups ? 1024 : 0);
-    for (sa = 3; sa >= 2; --sa) {
-      sb = (budget2 - sa * h.a_stage_bytes) / h.b_stage_bytes;
-      if (sb >= 3) break;
-    }
   }
-  PP_REQUIRE(sa >= 2 && sb >= 3, "conv_halo: patch %dx%d does not fit shared memory", h.BW, h.BH);
-  if (sb > MAX_SB) sb = MAX_SB;
-  if (!h.ups && sa == 3 && sb == MAX_SB && (budget - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
+  const int budget = SMEM_BUDGET - mt * h.out_stage_bytes;
+  PP_REQUIRE(halo_stages(budget, h.a_stage_bytes, h.b_stage_bytes, sa, sb), "conv_halo: patch %dx%d does not fit shared memory",
+             h.BW, h.BH);
+  if (sa == 3 && sb == MAX_SB && (budget - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
   h.SA = sa; h.SB = sb;
   if (h.tstore) {
     cuuint64_t dims[2] = {(cuuint64_t)p.Cout_g, (cuuint64_t)p.M_total};
@@ -830,23 +712,14 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
       dims[1] = (cuuint64_t)p.M_total; dims[2] = 1; dims[3] = 1;
       strides[1] = strides[2] = (cuuint64_t)p.M_total * s.cstride * 2;
     }
-    if (h.ups) {  // the tensor in memory is the half-resolution source; it lands unswizzled in the staging ring
-      dims[1] = (cuuint64_t)h.LW; dims[2] = (cuuint64_t)h.LH;
-      strides[1] = (cuuint64_t)h.LW * s.cstride * 2; strides[2] = (cuuint64_t)h.LH * h.LW * s.cstride * 2;
-      box[1] = (cuuint32_t)h.LBW; box[2] = (cuuint32_t)h.LBH;
-    }
     cuuint32_t es[4] = {1, 1, 1, 1};
     const CUresult r = enc(&h.tmap[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(s.ptr + s.coff), dims, strides, box,
-                           es, CU_TENSOR_MAP_INTERLEAVE_NONE, h.ups ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
+                           es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     PP_REQUIRE(r == CUDA_SUCCESS, "conv_halo: cuTensorMapEncodeTiled failed (%d) for segment %d (cstride=%d W=%d H=%d N=%d)",
                (int)r, i, s.cstride, p.W, p.H, p.N);
   }
   return PP_OK;
-}
-
-inline long long halo_total_tiles(const HaloParams& h) {
-  return (long long)h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * h.c.groups;
 }
 
 }  // namespace
@@ -856,25 +729,8 @@ int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   PP_TRY(halo_configure(pin, h, false));
   int num_sms = 0;
   PP_TRY(halo_num_sms(&num_sms));
-  const long long total_tiles = halo_total_tiles(h);
-  const size_t smem = (size_t)h.SA * h.a_stage_bytes + (size_t)h.SB * h.b_stage_bytes + 1024 + 1024 + 2 * (size_t)h.l_stage_bytes +
-                      (h.tstore ? (size_t)h.MT * h.out_stage_bytes + 1024 : 0) + 2 * ppconv::STG_BYTES;
-  const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(h.ups ? UPS_THREADS : NUM_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (h.ups) PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_halo_kernel<true>, h));
-  else PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_halo_kernel<false>, h));
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
+  const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, h.tstore ? h.MT * h.out_stage_bytes : 0).bytes;
+  return halo_launch(conv_halo_kernel, h, min(halo_total_tiles(h), num_sms), smem, stream);
 }
 
 // ---- multi-layer programs ------------------------------------------------------------------------------------------
@@ -902,13 +758,11 @@ void pp_prog_abort() {
   g_recorder = nullptr;
 }
 
-int pp_prog_eligible(const PPConvParams& p) { return pp_conv_halo_eligible(p) && !p.ups2x; }
-
 int pp_prog_record_conv(const PPConvParams& p) {
   PPProgRecorder* r = g_recorder;
   PP_REQUIRE(r != nullptr, "conv program: not recording");
   PP_REQUIRE(r->prog.n_layers < PROG_MAX_LAYERS, "conv program: more than %d layers", PROG_MAX_LAYERS);
-  PP_REQUIRE(pp_prog_eligible(p), "conv program: layer is not a stride-1 TMA halo-kernel convolution");
+  PP_REQUIRE(pp_conv_halo_eligible(p), "conv program: layer is not a stride-1 TMA halo-kernel convolution");
   const int li = r->prog.n_layers;
   PP_TRY(halo_configure(p, r->prog.layer[li], true));
   PP_REQUIRE(r->prog.layer[li].MT == 1 && r->prog.layer[li].c.BN <= 128, "conv program: layer tile %d x %d columns",
@@ -947,13 +801,9 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
       if (P.layer[i].a_stage_bytes > a_max) a_max = P.layer[i].a_stage_bytes;
       if (P.layer[i].b_stage_bytes > b_max) b_max = P.layer[i].b_stage_bytes;
     }
-  int sa = 3, sb = 0;
-  for (; sa >= 2; --sa) {
-    sb = (SMEM_BUDGET - sa * a_max) / b_max;
-    if (sb >= 3) break;
-  }
-  PP_REQUIRE(sa >= 2 && sb >= 3, "conv program: stages do not fit shared memory (A %d B, B %d B)", a_max, b_max);
-  if (sb > MAX_SB) sb = MAX_SB;
+  int sa = 0, sb = 0;
+  PP_REQUIRE(halo_stages(SMEM_BUDGET, a_max, b_max, sa, sb), "conv program: stages do not fit shared memory (A %d B, B %d B)",
+             a_max, b_max);
   P.SA = sa; P.SB = sb; P.a_stage_bytes = a_max; P.b_stage_bytes = b_max;
   P.counter = counter;
   P.base = *arrivals;
@@ -967,20 +817,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
   P.ts = (ts_mode && ts_printed < ts_mode) ? ts_dev : nullptr;
   const int grid = num_sms;
   *arrivals += (unsigned int)(P.n_layers * grid);
-  const size_t smem = (size_t)sa * a_max + (size_t)sb * b_max + 1024 + 1024 + 2 * ppconv::STG_BYTES;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_prog_kernel, P));
-  PP_CUDA_CHECK(cudaGetLastError());
+  PP_TRY(halo_launch(conv_prog_kernel, P, grid, halo_smem(nullptr, sa, a_max, sb, b_max, 0).bytes, stream));
   if (P.ts != nullptr) {      // debug: per-layer wall time of CTA 0 (serialises the stream)
     unsigned long long h[2 * PROG_MAX_LAYERS];
     PP_CUDA_CHECK(cudaStreamSynchronize(stream));
@@ -990,7 +827,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
     for (int i = 0; i < P.n_layers; ++i) {
       const HaloParams& L = P.layer[i];
       if (P.kind[i] == PROG_CONV)
-        fprintf(stderr, " | conv K=%d N=%d bn=%d mt=%d tiles=%lld: %.1f us (gap %.1f)", L.c.K_total, L.c.Cout_g, L.c.BN, L.MT,
+        fprintf(stderr, " | conv K=%d N=%d bn=%d mt=%d tiles=%d: %.1f us (gap %.1f)", L.c.K_total, L.c.Cout_g, L.c.BN, L.MT,
                 halo_total_tiles(L), (h[2 * i + 1] - h[2 * i]) / 1e3, i ? (h[2 * i] - h[2 * i - 1]) / 1e3 : 0.0);
       else
         fprintf(stderr, " | dcn: %.1f us (gap %.1f)", (h[2 * i + 1] - h[2 * i]) / 1e3, i ? (h[2 * i] - h[2 * i - 1]) / 1e3 : 0.0);

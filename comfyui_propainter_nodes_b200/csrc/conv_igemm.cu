@@ -231,7 +231,6 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   if (pp_prog_recording()) { g_last_kind = 'p'; return pp_prog_record_conv(p); }
   if (pp_conv_halo_eligible(p)) { g_last_kind = 'h'; return pp_launch_conv_halo(p, stream); }
   g_last_kind = 'i';
-  PP_REQUIRE(!p.ups2x, "conv: fused x2 upsampling needs the TMA halo kernel (stride 1, one input segment, even H and W)");
   for (int i = 0; i < p.nseg; ++i)
     PP_REQUIRE(p.seg[i].cvalid == 0, "conv: zero-extended input channels (cvalid=%d of %d) need the TMA halo kernel "
                "(stride 1, zero padding, Cin %% 64 == 0)", p.seg[i].cvalid, p.seg[i].cend - p.seg[i].cbegin);   // stride-1 k>1 layers: TMA halo-tile kernel

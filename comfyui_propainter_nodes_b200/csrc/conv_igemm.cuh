@@ -36,7 +36,6 @@ struct PPConvParams {
   int Cin;                // per-group input channels as seen by the kernel (multiple of 8)
   int kh, kw, sh, sw, ph, pw, dh, dw;
   int pad_replicate;      // 0: zeros outside, 1: clamp coordinates (replicate padding)
-  int ups2x;              // the input tensor is [N][H/2][W/2]: bilinear x2 (align_corners=True) on the fly (halo kernel only)
   int K_total;            // kh*kw*Cin
   int num_kc;             // ceil(K_total / 64)
   int M_total;            // N*OH*OW
@@ -71,7 +70,6 @@ struct PPProgRecorder;
 bool pp_prog_recording();
 int pp_prog_begin();
 void pp_prog_abort();
-int pp_prog_eligible(const PPConvParams& p);
 int pp_prog_record_conv(const PPConvParams& p);
 int pp_prog_record_dcn(const PPDcnArgs& a);
 int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stream);

@@ -85,111 +85,3 @@ __device__ __forceinline__ void dcn_sample_item(const PPDcnArgs& a, unsigned idx
 #pragma unroll
   for (int v = 0; v < CPG / 8; ++v) reinterpret_cast<uint4*>(d)[v] = reinterpret_cast<uint4*>(h)[v];
 }
-
-
-// ---- batched form: U independent items per thread in two phases, so that the offset loads of all U items are in flight
-// together and then all their corner gathers (one item alone is a chain of two dependent memory round trips; callers
-// with few threads per SM -- the multi-layer program kernel, the shared-memory tile sampler -- are latency-bound
-// without this).  SMEM_BOX: corners come from a staged box [BH][BW][QC] (see dcn_tiled.cu) when they fit in it.
-struct PPDcnItem {
-  long long m;      // pixel index over all images, -1 = no item
-  int n, g, k;
-  float py, px, mod;
-};
-
-template <bool COHERENT>
-__device__ __forceinline__ PPDcnItem dcn_item_setup(const PPDcnArgs& a, int n, int pix, int g, int k) {
-  PPDcnItem it;
-  const int W = a.W;
-  const int x = pix % W, y = pix / W;
-  it.n = n; it.g = g; it.k = k;
-  it.m = (long long)n * a.H * W + pix;
-  const __half* o = a.offs + it.m * a.offs_cs;
-  const int gk = g * 9 + k;
-  float dy = a.max_mag * tanhf(dcn_ldh<COHERENT>(o + 2 * gk));
-  float dx = a.max_mag * tanhf(dcn_ldh<COHERENT>(o + 2 * gk + 1));
-  if (a.flow != nullptr) {
-    dx += dcn_ldh<COHERENT>(a.flow + it.m * a.flow_cs + a.flow_co);
-    dy += dcn_ldh<COHERENT>(a.flow + it.m * a.flow_cs + a.flow_co + 1);
-  }
-  it.mod = 1.f / (1.f + __expf(-dcn_ldh<COHERENT>(o + 288 + gk)));
-  it.py = (float)(y - 1 + k / 3) + dy;
-  it.px = (float)(x - 1 + k % 3) + dx;
-  return it;
-}
-
-// corner gathers of one item into `q` ([4 corners][CPG/8] vectors, zero where the corner does not contribute) and the
-// bilinear weights into w[4]; box == nullptr: always from global memory
-template <int CPG, bool COHERENT>
-__device__ __forceinline__ void dcn_item_gather(const PPDcnArgs& a, const PPDcnItem& it, const uint8_t* box, int by0, int bx0,
-                                                int BH, int BW, int QC, int gq, uint4 (&q)[4][CPG / 8], float (&w)[4]) {
-  const int H = a.H, W = a.W;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    w[c] = 0.f;
-#pragma unroll
-    for (int v = 0; v < CPG / 8; ++v) q[c][v] = make_uint4(0, 0, 0, 0);
-  }
-  if (it.m < 0 || !(it.py > -1.f && it.py < (float)H && it.px > -1.f && it.px < (float)W)) return;
-  const float fy = floorf(it.py), fx = floorf(it.px);
-  const int yy0 = (int)fy, xx0 = (int)fx;
-  const float ay = it.py - fy, ax = it.px - fx;
-  const int ry = yy0 - by0, rx = xx0 - bx0;
-  if (box != nullptr && ry >= 0 && rx >= 0 && ry + 1 < BH && rx + 1 < BW) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      w[c] = ((c >> 1) ? ay : 1.f - ay) * ((c & 1) ? ax : 1.f - ax);
-      const uint4* vp = reinterpret_cast<const uint4*>(box + ((ry + (c >> 1)) * BW + rx + (c & 1)) * (QC * 2) + gq * (CPG * 2));
-#pragma unroll
-      for (int v = 0; v < CPG / 8; ++v) q[c][v] = vp[v];
-    }
-    return;
-  }
-  const int ch = it.g * CPG;  // channel inside cat(x0, x1)
-  const __half* src;
-  int cs;
-  if (ch < a.C0) { src = a.x0 + a.x0_co + ch; cs = a.x0_cs; }
-  else { src = a.x1 + a.x1_co + (ch - a.C0); cs = a.x1_cs; }
-  src += (long long)it.n * H * W * cs;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    const int yy = yy0 + (c >> 1), xx = xx0 + (c & 1);
-    if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
-    w[c] = ((c >> 1) ? ay : 1.f - ay) * ((c & 1) ? ax : 1.f - ax);
-    const uint4* vp = reinterpret_cast<const uint4*>(src + ((long long)yy * W + xx) * cs);
-#pragma unroll
-    for (int v = 0; v < CPG / 8; ++v) q[c][v] = COHERENT ? __ldcg(vp + v) : vp[v];
-  }
-}
-
-// blend in the corner order of dcn_sample_item (bit-identical results), modulate, store
-template <int CPG>
-__device__ __forceinline__ void dcn_item_store(const PPDcnArgs& a, const PPDcnItem& it, const uint4 (&q)[4][CPG / 8],
-                                               const float (&w)[4]) {
-  if (it.m < 0) return;
-  float acc[CPG];
-#pragma unroll
-  for (int i = 0; i < CPG; ++i) acc[i] = 0.f;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    // a skipped corner (outside the image) has w == 0 and q == 0: adding +0 leaves acc unchanged
-#pragma unroll
-    for (int v = 0; v < CPG / 8; ++v) {
-      const __half2* hq = reinterpret_cast<const __half2*>(&q[c][v]);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = __half22float2(hq[e]);
-        acc[v * 8 + 2 * e] += w[c] * f.x;
-        acc[v * 8 + 2 * e + 1] += w[c] * f.y;
-      }
-    }
-  }
-  __half* d = a.cols + it.m * (long long)(9 * a.C) + it.k * a.C + it.g * CPG;
-#pragma unroll
-  for (int v = 0; v < CPG / 8; ++v) {
-    __align__(16) __half2 h[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(it.mod * acc[v * 8 + 2 * e], it.mod * acc[v * 8 + 2 * e + 1]);
-    reinterpret_cast<uint4*>(d)[v] = *reinterpret_cast<uint4*>(h);
-  }
-}

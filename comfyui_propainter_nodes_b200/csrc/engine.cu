@@ -56,17 +56,6 @@ PPConvCall& PPConvCall::geom(int sh, int sw, int ph, int pw, int dh, int dw, int
   return *this;
 }
 
-int pp_fuse_upsample() {
-  // read on every call (a getenv per deconv layer is noise) so tests can exercise both paths in one process
-  const char* s = getenv("PP_FUSE_UPSAMPLE");
-  return (s != nullptr && atoi(s) != 0) ? 1 : 0;
-}
-
-PPConvCall& PPConvCall::upsampled2x() {
-  p.ups2x = 1;
-  return *this;
-}
-
 PPConvCall& PPConvCall::out(void* ptr, int cs, int co, int fp32, int gstep) {
   p.out = ptr; p.out_cstride = cs; p.out_coff = co; p.out_fp32 = fp32; p.out_gstep = gstep;
   return *this;

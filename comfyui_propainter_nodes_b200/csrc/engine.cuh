@@ -117,7 +117,6 @@ struct PPConvCall {
   PPConvCall(PPEngine& e, const std::string& name, int N, int H, int W);
   PPConvCall& in(const __half* ptr, int cs, int co, int channels, int gstep = 0);
   PPConvCall& geom(int sh, int sw, int ph, int pw, int dh = 1, int dw = 1, int replicate = 0);
-  PPConvCall& upsampled2x();   // the tensor given to in() is [N][H/2][W/2]: bilinear x2 (align_corners) fused into the conv
   PPConvCall& out(void* ptr, int cs, int co, int fp32 = 0, int gstep = 0);
   PPConvCall& act(int act1, float slope = 0.f, float scale = 1.f, int act2 = PP_ACT_NONE);
   PPConvCall& residual(const __half* ptr, int cs, int co);
@@ -125,13 +124,6 @@ struct PPConvCall {
   PPConvCall& gru_h(const __half* h, int h_cs, int h_co, const __half* z, int z_cs, int z_co);
   int run(cudaStream_t st);
 };
-
-// Deconv layers (bilinear x2 + 3x3 conv).  Default: upsample2x_ac materialises the upsampled tensor, then the conv.
-// PP_FUSE_UPSAMPLE=1: ONE launch of the halo kernel's fused-upsample variant (the 128 producer threads interpolate the
-// low-res patch into the A stage; the 4x tensor never exists).  Correct (parity-tested) but measured slower at C2 --
-// the interpolation (2,592 16-byte items per 64-channel chunk) outlasts the MMAs of a 64..128-column tile
-// (gen.decoder.4: 6.8 ms fused vs 4.1 + 1.9 ms) -- so it is opt-in until the producer gets wider.
-int pp_fuse_upsample();
 
 void pp_build_ring_indices(int nh, int nw, std::vector<int>& out);
 

@@ -48,8 +48,6 @@ namespace {
 
 int deconv(PPEngine& e, const std::string& name, const __half* x, int n, int h, int w, int cin, __half* up,
            __half* out, int cout, int out_cs, int act, float slope, cudaStream_t st) {
-  if (pp_fuse_upsample())
-    return PPConvCall(e, name, n, 2 * h, 2 * w).in(x, cin, 0, cin).upsampled2x().out(out, out_cs, 0).act(act, slope).run(st);
   PP_TRY(pp_k_upsample2x(x, cin, 0, up, cin, 0, n, h, w, cin, st));
   e.launches++;
   return PPConvCall(e, name, n, 2 * h, 2 * w).in(up, cin, 0, cin).out(out, out_cs, 0).act(act, slope).run(st);

@@ -53,10 +53,6 @@ int pp_k_rfc_combine(const __half* pred, int pred_cs, long long pred_tstride_pix
 int pp_k_dcn_sample(const __half* x0, int x0_cs, int x0_co, int C0, const __half* x1, int x1_cs, int x1_co, int C1,
                     const __half* offs, int offs_cs, const __half* flow, int flow_cs, int flow_co, float max_mag,
                     __half* cols, int N, int H, int W, cudaStream_t st);
-struct PPDcnArgs;
-// dcn_tiled.cu: the same sampling with the source tile staged in shared memory by TMA; *handled = 0 when not applicable
-int pp_k_dcn_sample_tiled(const PPDcnArgs& a, int flow_margin, cudaStream_t st, int* handled);
-int pp_k_dcn_sample_plain(const PPDcnArgs& a, cudaStream_t st);
 int pp_k_featprop_cond(const __half* cur, int cur_cs, const __half* prop, int prop_cs, const __half* flow_prop,
                        const __half* flow_check, const __half* mask2, int mask_cs, __half* cond, int cond_cs, int N,
                        int H, int W, int C, cudaStream_t st);

@@ -538,27 +538,8 @@ int pp_k_dcn_sample(const __half* x0, int x0_cs, int x0_co, int C0, const __half
   a.flow = flow; a.flow_cs = flow_cs; a.flow_co = flow_co;
   a.max_mag = max_mag; a.cols = cols; a.C = C; a.N = N; a.H = H; a.W = W;
   if (pp_prog_recording()) return pp_prog_record_dcn(a);     // multi-layer program (conv_halo.cu): runs inside it
-  {
-    // opt-in (PP_DCN_TILED=1): source tiles staged in shared memory by TMA (dcn_tiled.cu).  Bit-identical, but measured
-    // no faster than the plain sampler (35 vs 36 us at the flow-completion size, 97 vs 102 us at the generator's): the
-    // sampler is bound by L1 wavefronts of its uncoalesced accesses, the offsets / stores keep that cost
-    const char* s = getenv("PP_DCN_TILED");       // read per call: tests compare both samplers in one process
-    if (s != nullptr && atoi(s) != 0) {
-      int handled = 0;
-      PP_TRY(pp_k_dcn_sample_tiled(a, 3, st, &handled));
-      if (handled) return PP_OK;
-    }
-  }
-  return pp_k_dcn_sample_plain(a, st);
-}
-
-int pp_k_dcn_sample_plain(const PPDcnArgs& a, cudaStream_t st) {
-  PP_REQUIRE(a.C == 128 || a.C == 256, "dcn_sample: C=%d must be 128 or 256 (16 offset groups)", a.C);
-  if ((long long)a.N * a.H * a.W == 0) return PP_OK;
-  PP_REQUIRE(a.N <= 65535 && (long long)a.H * a.W * 144 < (1LL << 31), "dcn_sample: %d images of %dx%d exceed the grid limits",
-             a.N, a.W, a.H);
-  const dim3 grid(pp_ceil_div(a.H * a.W * 144, TPB), a.N);
-  if (a.C == 128) dcn_sample<8><<<grid, TPB, 0, st>>>(a);
+  const dim3 grid(pp_ceil_div(H * W * 144, TPB), N);
+  if (C == 128) dcn_sample<8><<<grid, TPB, 0, st>>>(a);
   else dcn_sample<16><<<grid, TPB, 0, st>>>(a);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;

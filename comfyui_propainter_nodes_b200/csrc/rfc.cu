@@ -213,32 +213,18 @@ int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows
     PP_TRY(pp_alloc(e, &pred, (size_t)Nd * HW * 2, "rfc pred"));
     PP_TRY(PPConvCall(e, "rfc.decoder2.0", Nd, h8, w8).in(fused, 128, 0, 128).out(d2a, 128, 0)
                .act(PP_ACT_LRELU, 0.2f).run(st));
-    const bool fuse = pp_fuse_upsample() != 0;   // deconv = bilinear x2 + 3x3 conv in one launch (halo kernel, UPS variant)
-    if (fuse) {
-      PP_TRY(PPConvCall(e, "rfc.decoder2.deconv", Nd, h4, w4).in(d2a, 128, 0, 128).upsampled2x().out(d2, 64, 0)
-                 .act(PP_ACT_LRELU, 0.2f).residual(e1own, 64, 0).run(st));
-    } else {
-      PP_TRY(pp_k_upsample2x(d2a, 128, 0, up, 128, 0, Nd, h8, w8, 128, st));
-      PP_TRY(PPConvCall(e, "rfc.decoder2.deconv", Nd, h4, w4).in(up, 128, 0, 128).out(d2, 64, 0)
-                 .act(PP_ACT_LRELU, 0.2f).residual(e1own, 64, 0).run(st));
-    }
+    // deconv = bilinear x2 (materialised in `up`) + 3x3 conv
+    PP_TRY(pp_k_upsample2x(d2a, 128, 0, up, 128, 0, Nd, h8, w8, 128, st));
+    PP_TRY(PPConvCall(e, "rfc.decoder2.deconv", Nd, h4, w4).in(up, 128, 0, 128).out(d2, 64, 0)
+               .act(PP_ACT_LRELU, 0.2f).residual(e1own, 64, 0).run(st));
     PP_TRY(PPConvCall(e, "rfc.decoder1.0", Nd, h4, w4).in(d2, 64, 0, 64).out(d1a, 64, 0).act(PP_ACT_LRELU, 0.2f).run(st));
-    if (fuse) {
-      PP_TRY(PPConvCall(e, "rfc.decoder1.deconv", Nd, h2, w2).in(d1a, 64, 0, 64).upsampled2x().out(d1, 32, 0)
-                 .act(PP_ACT_LRELU, 0.2f).run(st));
-    } else {
-      PP_TRY(pp_k_upsample2x(d1a, 64, 0, up, 64, 0, Nd, h4, w4, 64, st));
-      PP_TRY(PPConvCall(e, "rfc.decoder1.deconv", Nd, h2, w2).in(up, 64, 0, 64).out(d1, 32, 0)
-                 .act(PP_ACT_LRELU, 0.2f).run(st));
-    }
+    PP_TRY(pp_k_upsample2x(d1a, 64, 0, up, 64, 0, Nd, h4, w4, 64, st));
+    PP_TRY(PPConvCall(e, "rfc.decoder1.deconv", Nd, h2, w2).in(up, 64, 0, 64).out(d1, 32, 0)
+               .act(PP_ACT_LRELU, 0.2f).run(st));
     PP_TRY(PPConvCall(e, "rfc.upsample.0", Nd, h2, w2).in(d1, 32, 0, 32).out(u0, 32, 0).act(PP_ACT_LRELU, 0.2f).run(st));
-    if (!fuse) PP_TRY(pp_k_upsample2x(u0, 32, 0, up, 32, 0, Nd, h2, w2, 32, st));
+    PP_TRY(pp_k_upsample2x(u0, 32, 0, up, 32, 0, Nd, h2, w2, 32, st));
     // 32 -> 2 tail (channels zero-extended to 64 by TMA, 16-column N tile)
-    if (fuse) {
-      PP_TRY(PPConvCall(e, "rfc.upsample.deconv", Nd, H, W).in(u0, 32, 0, 32).upsampled2x().out(pred, 2, 0).run(st));
-    } else {
-      PP_TRY(PPConvCall(e, "rfc.upsample.deconv", Nd, H, W).in(up, 32, 0, 32).out(pred, 2, 0).run(st));
-    }
+    PP_TRY(PPConvCall(e, "rfc.upsample.deconv", Nd, H, W).in(up, 32, 0, 32).out(pred, 2, 0).run(st));
     e.launches += 3;
 
     // ---- combine_flow (:389-400) and un-flip, rows of the owned frames --------------------------------

@@ -60,7 +60,6 @@ _SIGNATURES = {
     "pp_op_conv": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _F, _VP, _VP, _VP]),
     "pp_op_corr_lookup": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
     "pp_op_imgprop_step": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP]),
-    "pp_op_dcn_sample": (_I, [_VP, _VP, _VP, _VP, _F, _VP, _I, _I, _I, _I, _I, _VP]),
     "pp_op_attention": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
 }
 
@@ -697,14 +696,6 @@ class Engine:
         self._check(self.lib.pp_op_imgprop_step(self.h, _ptr(cur4), _ptr(prop4), _ptr(out), _ptr(flow_prop),
                                                 _ptr(flow_check), H, W, self._stream()))
         return out
-
-    def op_dcn_sample(self, x, offs, flow, max_mag: float, tiled: bool):
-        """x [N,H,W,C] fp16, offs [N,H,W,432] fp16, flow [N,H,W,2] fp16 or None -> cols [N*H*W, 9*C] fp16."""
-        N, H, W, C = x.shape
-        cols = torch.empty(N * H * W, 9 * C, device=self.device, dtype=torch.float16)
-        self._check(self.lib.pp_op_dcn_sample(self.h, _ptr(x), _ptr(offs), _ptr(flow), float(max_mag), _ptr(cols), N, H, W, C,
-                                              int(tiled), self._stream()))
-        return cols
 
     def op_attention(self, qkv, pkv, win_flags, t, gh, gw, n_pool, parity):
         out = torch.zeros(t, gh, gw, 512, device=self.device, dtype=torch.float16)

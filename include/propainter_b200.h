@@ -152,10 +152,6 @@ PP_API int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const 
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream);
 PP_API int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* prop_in4_f16, void* prop_out4_f16,
                        const void* flow_prop_f16, const void* flow_check_f16, int H, int W, void* stream);
-/* Modulated deformable sampling -> columns [N*H*W][9*C]: x [N,H,W,C] (C = 128, or 256 = two 128-channel halves),
- * offs [N,H,W,432] raw offset-head output, flow [N,H,W,2] (dx,dy) or NULL; tiled = 1: TMA-staged sampler. */
-PP_API int pp_op_dcn_sample(pp_handle h, const void* x_f16, const void* offs_f16, const void* flow_f16, float max_mag,
-                            void* cols_f16, int N, int H, int W, int C, int tiled, void* stream);
 PP_API int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,
                     int t, int gh, int gw, int n_pool, int parity, void* stream);
 

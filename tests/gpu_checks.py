@@ -396,39 +396,10 @@ def check_composite_exact():
     return res
 
 
-def check_dcn_samplers(timing=False):
-    """TMA-staged tiled sampler == plain L2 sampler, bit for bit (same arithmetic in the same order), on the two shapes
-    of the pipeline: C=256 / |offset| <= 5 (flow completion) and C=128 / 3*tanh + flow (generator), with offsets that also
-    leave the staged box (large flows) and the image."""
-    eng = bare_engine()
-    g = torch.Generator().manual_seed(9)
-    res = {}
-    for tag, (N, H, W, C, mag, fscale) in {"rfc": (2, 45, 80, 256, 5.0, None), "gen": (3, 90, 160, 128, 3.0, 2.5),
-                                           "gen_big_flow": (2, 40, 56, 128, 3.0, 12.0)}.items():
-        x = torch.randn(N, H, W, C, generator=g).half().to(DEV)
-        offs = (torch.randn(N, H, W, 432, generator=g) * 1.5).half().to(DEV)
-        flow = None if fscale is None else (torch.randn(N, H, W, 2, generator=g) * fscale).half().to(DEV)
-        a = eng.op_dcn_sample(x, offs, flow, mag, False)
-        b = eng.op_dcn_sample(x, offs, flow, mag, True)
-        torch.cuda.synchronize()
-        res[tag] = dict(mismatch=int((a != b).sum()), nonzero=float((a != 0).float().mean()), nan=bool(torch.isnan(b.float()).any()))
-        if timing:
-            for name, tl in (("plain", False), ("tiled", True)):
-                s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                eng.op_dcn_sample(x, offs, flow, mag, tl)
-                s.record()
-                for _ in range(20):
-                    eng.op_dcn_sample(x, offs, flow, mag, tl)
-                e.record()
-                torch.cuda.synchronize()
-                res[tag][name + "_us"] = s.elapsed_time(e) / 20 * 1000
-    return res
-
-
 def check_step_variants():
-    """The recurrent propagation steps have three execution variants -- multi-layer program kernel (default), one launch
-    per layer with the TMA-staged deformable sampler, one launch per layer with the plain L2 sampler -- that perform the
-    same arithmetic in the same order: outputs must be bit-identical (flow completion, generator window)."""
+    """The recurrent propagation steps have two execution variants -- multi-layer program kernel (default) and one launch
+    per layer -- that perform the same arithmetic in the same order: outputs must be bit-identical (flow completion,
+    generator window)."""
     import os
     m = full_models()
     eng = m.flow_model.engine
@@ -440,11 +411,10 @@ def check_step_variants():
     wb = torch.zeros(t - 1, 2, H, W)
     wf[:l_t - 1], wb[:l_t - 1] = c["flows"][0][0], c["flows"][1][0]
     outs = {}
-    keep = {k: os.environ.get(k) for k in ("PP_PROG", "PP_DCN_TILED")}
+    keep = os.environ.get("PP_PROG")
     try:
-        for tag, env in (("program", {"PP_PROG": "1", "PP_DCN_TILED": "1"}), ("tiled", {"PP_PROG": "0", "PP_DCN_TILED": "1"}),
-                         ("plain", {"PP_PROG": "0", "PP_DCN_TILED": "0"})):
-            os.environ.update(env)
+        for tag, prog in (("program", "1"), ("plain", "0")):
+            os.environ["PP_PROG"] = prog
             of, ob = eng.flow_complete(ff[0].to(DEV), fb[0].to(DEV), masks[0].to(DEV))
             eng.gen_begin(c["frames"][0].to(DEV), c["masks_in"][0].to(DEV), c["masks_upd"][0].to(DEV), wf.to(DEV), wb.to(DEV))
             pred = eng.gen_window(list(range(t)), l_t)
@@ -452,17 +422,13 @@ def check_step_variants():
             torch.cuda.synchronize()
             outs[tag] = (of.clone(), ob.clone(), pred.clone())
     finally:
-        for k, v in keep.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-    res = {}
-    for tag in ("program", "tiled"):
-        # lane 3 of the prediction tensor is never written (3 output channels in a 4-wide pixel): compare rgb only
-        res[tag + "_vs_plain"] = [int((a[..., :3] != b[..., :3]).sum()) if a.dim() == 4 and a.shape[-1] == 4 else int((a != b).sum())
-                                  for a, b in zip(outs[tag], outs["plain"])]
-    return res
+        if keep is None:
+            os.environ.pop("PP_PROG", None)
+        else:
+            os.environ["PP_PROG"] = keep
+    # lane 3 of the prediction tensor is never written (3 output channels in a 4-wide pixel): compare rgb only
+    return {"program_vs_plain": [int((a[..., :3] != b[..., :3]).sum()) if a.dim() == 4 and a.shape[-1] == 4 else int((a != b).sum())
+                                 for a, b in zip(outs["program"], outs["plain"])]}
 
 
 def check_small_workspace_fallback():
@@ -507,8 +473,7 @@ def main():
                ("e2e", lambda: check_e2e(golden)), ("c1_node", lambda: check_c1_node(golden2)),
                ("raft20", lambda: check_raft20(golden2)), ("chunked", lambda: check_chunked(golden2)),
                ("outpaint_node", lambda: check_outpaint_node(golden2)), ("composite_exact", check_composite_exact),
-               ("small_workspace", check_small_workspace_fallback), ("step_variants", check_step_variants),
-               ("dcn_samplers", lambda: check_dcn_samplers(True))]
+               ("small_workspace", check_small_workspace_fallback), ("step_variants", check_step_variants)]
     for name, fn in checks:
         if only and not any(o in name for o in only):
             continue

@@ -177,11 +177,3 @@ def test_device_preprocessing_is_bit_exact(C):
         assert np.array_equal(orig2.cpu().numpy(), np.stack(orig))
     u8 = torch.randint(0, 256, (2, 8, 8, 3), dtype=torch.uint8)
     assert torch.equal(eng.postprocess(u8.to(C.DEV)).cpu(), u8.float() / 255.0)
-
-
-def test_fused_upsample_deconv_matches_reference(C, golden, monkeypatch):
-    """PP_FUSE_UPSAMPLE=1: the deconv layers (bilinear x2 + conv) of the flow-completion decoder run as one launch of
-    the halo kernel's fused-upsample variant; same bound as the default path."""
-    monkeypatch.setenv("PP_FUSE_UPSAMPLE", "1")
-    for k, s in C.check_rfc(golden).items():
-        assert not s["nan"] and s["max_abs"] < 0.02, (k, s)

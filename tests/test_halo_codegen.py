@@ -12,7 +12,7 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "comfyui_propainter_nodes_b200", "csrc")
-KERNEL = "conv_halo_kernelILb0E"     # mangled conv_halo_kernel<false>
+KERNEL = "16conv_halo_kernelENS_10HaloParamsE"     # mangled conv_halo_kernel(HaloParams), anonymous namespace
 
 
 def _cuda_tool(name):
@@ -43,7 +43,7 @@ def test_halo_kernel_has_no_wgmma_serialization_warnings(halo_build):
     assert not bad, "\n".join(bad[:8])
 
 
-def test_halo_kernel_sass_waits_once_per_commit_group(halo_build):
+def test_conv_halo_kernel_sass_waits_once_per_commit_group(halo_build):
     cuobjdump = _cuda_tool("cuobjdump")
     if cuobjdump is None:
         pytest.skip("cuobjdump not found")
@@ -51,7 +51,7 @@ def test_halo_kernel_sass_waits_once_per_commit_group(halo_build):
     sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
     funcs = re.split(r"\n\s*Function : ", sass)
     body = next((f for f in funcs if f.startswith("_Z") and KERNEL in f.split("\n", 1)[0]), None)
-    assert body is not None, "conv_halo_kernel<false> not found in the SASS"
+    assert body is not None, "conv_halo_kernel not found in the SASS"
     hgmma = len(re.findall(r"\bHGMMA\.", body))
     depbar = len(re.findall(r"\bWARPGROUP\.DEPBAR", body))
     assert hgmma > 0
