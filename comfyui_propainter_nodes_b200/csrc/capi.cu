@@ -160,7 +160,15 @@ int pp_raft_bidir(pp_handle h, const float* frames, int T, int H, int W, int ite
   PP_HANDLE(h);
   PP_REQUIRE(frames && flows_f && flows_b, "pp_raft_bidir: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_raft(e, frames, T, H, W, iters, flows_f, flows_b, as_stream(stream));
+  return pp_stage_raft(e, frames, T, H, W, iters, flows_f, flows_b, false, as_stream(stream));
+}
+
+int pp_raft_bidir_fp32(pp_handle h, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
+                       void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(frames && flows_f && flows_b, "pp_raft_bidir_fp32: null pointer");
+  ArenaGuard guard(e.arena);
+  return pp_stage_raft(e, frames, T, H, W, iters, flows_f, flows_b, true, as_stream(stream));
 }
 
 int pp_flow_complete(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T, int H,

@@ -191,6 +191,111 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
     }
 }
 
+// ---- split-tf32 form (PPConvParams::split): fp32 [hi | lo] operands, see conv_igemm.cuh
+// hi = x rounded to tf32 (10 explicit mantissa bits, nearest, ties away), lo = x - hi (exact in fp32)
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+// 16 consecutive channels x = hi + lo of a split tensor (hi at src, lo `lo` floats further)
+__device__ __forceinline__ void load16_split(const float* src, int lo, int nvalid, bool vec, float (&r)[16]) {
+  if (vec && nvalid == 16) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float4 h = reinterpret_cast<const float4*>(src)[i], l = reinterpret_cast<const float4*>(src + lo)[i];
+      r[4 * i] = h.x + l.x; r[4 * i + 1] = h.y + l.y; r[4 * i + 2] = h.z + l.z; r[4 * i + 3] = h.w + l.w;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) r[i] = i < nvalid ? src[i] + src[lo + i] : 0.f;
+  }
+}
+__device__ __forceinline__ void store16_split(float* dst, int lo, int nvalid, bool vec, const float (&v)[16]) {
+  float h[16], l[16];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) { h[i] = tf32_rna(v[i]); l[i] = v[i] - h[i]; }
+  if (vec && nvalid == 16) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      reinterpret_cast<float4*>(dst)[i] = make_float4(h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
+      reinterpret_cast<float4*>(dst + lo)[i] = make_float4(l[4 * i], l[4 * i + 1], l[4 * i + 2], l[4 * i + 3]);
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (i < nvalid) { dst[i] = h[i]; dst[lo + i] = l[i]; }
+  }
+}
+
+// conv_epilogue16 of the split-tf32 form: the same three epilogue kinds; auxiliary operands are read as hi + lo, results
+// are written as hi / lo pairs (or plain fp32 with out_fp32).
+__device__ __forceinline__ void conv_epilogue16_split(const PPConvParams& p, const float (&acc)[16], long long mrow, int g,
+                                                      int ng0, bool vec) {
+  const int nvalid = min(16, p.Cout_g - ng0);
+  float v[16];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) v[i] = acc[i];
+  if (p.bias != nullptr) {
+    const float* bp = p.bias + g * p.Cout_g + ng0;
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (i < nvalid) v[i] += __ldg(bp + i);
+  }
+  const float* aux0 = reinterpret_cast<const float*>(p.aux0);
+  const float* aux1 = reinterpret_cast<const float*>(p.aux1);
+  float* out = reinterpret_cast<float*>(p.out);
+  if (p.epi == PP_EPI_STD) {
+    act16(v, p.act1, p.slope);
+    if (p.scale != 1.f) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[i] *= p.scale;
+    }
+    if (aux0 != nullptr) {
+      float r[16];
+      load16_split(aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, p.aux0_lo, nvalid, vec, r);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[i] += r[i];
+    }
+    act16(v, p.act2, p.slope);
+    float* dst = out + mrow * p.out_cstride + p.out_coff + (long long)g * p.out_gstep + ng0;
+    if (p.out_fp32) {
+      if (vec && nvalid == 16) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          reinterpret_cast<float4*>(dst)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+          if (i < nvalid) dst[i] = v[i];
+      }
+    } else {
+      store16_split(dst, p.out_lo, nvalid, vec, v);
+    }
+  } else if (p.epi == PP_EPI_GRU_ZR) {
+    const int half_c = p.Cout_g >> 1;
+    act16_t<PP_ACT_SIGMOID>(v, 0.f);
+    if (ng0 < half_c) {
+      store16_split(out + mrow * p.out_cstride + p.out_coff + ng0, p.out_lo, nvalid, vec, v);
+    } else {
+      const int c = ng0 - half_c;
+      float h[16];
+      load16_split(aux0 + mrow * p.aux0_cstride + p.aux0_coff + c, p.aux0_lo, nvalid, vec, h);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[i] *= h[i];
+      store16_split(reinterpret_cast<float*>(p.out2) + mrow * p.out2_cstride + p.out2_coff + c, p.out2_lo, nvalid, vec, v);
+    }
+  } else {  // PP_EPI_GRU_H
+    float h[16], z[16];
+    load16_split(aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, p.aux0_lo, nvalid, vec, h);
+    load16_split(aux1 + mrow * p.aux1_cstride + p.aux1_coff + ng0, p.aux1_lo, nvalid, vec, z);
+    act16_t<PP_ACT_TANH>(v, 0.f);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) v[i] = (1.f - z[i]) * h[i] + z[i] * v[i];
+    store16_split(out + mrow * p.out_cstride + p.out_coff + ng0, p.out_lo, nvalid, vec, v);
+  }
+}
+
 // ---- accumulator hand-off for the wgmma kernels
 // A warpgroup's m64 x N accumulator is spread over its 128 threads in the wgmma fragment layout (pp_common.cuh); the
 // epilogue wants 16 consecutive channels of one pixel per thread.  Per 32-column chunk the warpgroup writes its
@@ -226,17 +331,28 @@ __device__ __forceinline__ void drain_acc(const float (&acc)[N / 2], float* stg,
   }
 }
 
-// conv_epilogue16 on 16 staged accumulators
+// conv_epilogue16 (SPLIT: conv_epilogue16_split) on 16 staged accumulators
+template <bool SPLIT = false>
 __device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const float* src, long long mrow, int g, int ng0,
                                                     uint4* sm0, uint4* sm1) {
-  uint32_t raw[16];
+  if constexpr (SPLIT) {
+    float acc[16];
 #pragma unroll
-  for (int i = 0; i < 16; i += 4) {
-    const float4 v = *reinterpret_cast<const float4*>(src + i);
-    raw[i] = __float_as_uint(v.x); raw[i + 1] = __float_as_uint(v.y);
-    raw[i + 2] = __float_as_uint(v.z); raw[i + 3] = __float_as_uint(v.w);
+    for (int i = 0; i < 16; i += 4) {
+      const float4 v = *reinterpret_cast<const float4*>(src + i);
+      acc[i] = v.x; acc[i + 1] = v.y; acc[i + 2] = v.z; acc[i + 3] = v.w;
+    }
+    conv_epilogue16_split(p, acc, mrow, g, ng0, p.vec_ok != 0);
+  } else {
+    uint32_t raw[16];
+#pragma unroll
+    for (int i = 0; i < 16; i += 4) {
+      const float4 v = *reinterpret_cast<const float4*>(src + i);
+      raw[i] = __float_as_uint(v.x); raw[i + 1] = __float_as_uint(v.y);
+      raw[i + 2] = __float_as_uint(v.z); raw[i + 3] = __float_as_uint(v.w);
+    }
+    conv_epilogue16(p, raw, mrow, g, ng0, p.epi, p.vec_ok != 0, nullptr, sm0, sm1);
   }
-  conv_epilogue16(p, raw, mrow, g, ng0, p.epi, p.vec_ok != 0, nullptr, sm0, sm1);
 }
 
 // f(IntC<BN>{}) for the runtime tile width bn (a multiple of 16, at most MAX_N)

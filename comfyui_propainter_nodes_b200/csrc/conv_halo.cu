@@ -17,6 +17,10 @@
 // Warp roles (384 threads, one persistent CTA per SM): warpgroups 0-1 consumers (wgmma into register accumulators,
 // then the fused epilogue of conv_epilogue.cuh -> global), warp 8 patch producer (TMA), warp 9 weight producer (bulk
 // copy).  MT == 1: warpgroup w owns pixel rows 64w..64w+63 of the sub-tile; MT == 2: warpgroup w owns sub-tile w.
+//
+// conv_halo_tf32_kernel is the split-tf32 form (PPConvParams::split, see conv_igemm.cuh): the byte geometry is the same
+// (a 128-byte swizzled K-chunk row holds 32 fp32 channels, each chunk is 4 wgmmas m64nNk8 with the same 32-byte
+// descriptor step), so the tap views, rings and producers are shared; only the MMA instruction and the epilogue differ.
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -39,7 +43,7 @@ constexpr int SMEM_BUDGET = 186 * 1024;
 
 struct HaloParams {
   PPConvParams c;
-  CUtensorMap tmap[4];
+  CUtensorMap tmap[PP_MAX_SEGS];
   int MT;            // sub-tiles (128 pixels each) per CTA tile
   int BW, BH;        // patch size in pixels
   int tiles_x, tiles_y, n_tiles;
@@ -139,13 +143,17 @@ __device__ __forceinline__ uint8_t* halo_smem_base() {
 __host__ __device__ constexpr int halo_max_tps(int bn) { return 128 / bn > 1 ? 128 / bn : 1; }
 
 // One filter tap: 4 k-steps of 16 channels for each m64 block, then the descriptors move on to the next tap.
-template <int BN, int MB>
+// TF32: the split-tf32 form (4 k-steps of 8 fp32 channels, the same 32-byte descriptor step).
+template <int BN, int MB, bool TF32>
 __device__ __forceinline__ void halo_tap(float (&acc)[MB][BN / 2], uint64_t (&adesc)[MB], uint64_t& bdesc, uint32_t& accum,
                                          int& kx, int kw, uint32_t step_x, uint32_t step_row, uint32_t tap16) {
 #pragma unroll
   for (int k = 0; k < 4; ++k)
 #pragma unroll
-    for (int b = 0; b < MB; ++b) ppx::wgmma_f16<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (accum | k) != 0 ? 1u : 0u);
+    for (int b = 0; b < MB; ++b) {
+      if constexpr (TF32) ppx::wgmma_tf32<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (accum | k) != 0 ? 1u : 0u);
+      else ppx::wgmma_f16<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (accum | k) != 0 ? 1u : 0u);
+    }
   accum = 1u;
   bdesc += tap16;
   const uint32_t step = ++kx == kw ? step_row : step_x;
@@ -160,25 +168,25 @@ __device__ __forceinline__ void halo_tap(float (&acc)[MB][BN / 2], uint64_t (&ad
 // joins (C7519 / C7520) and makes every wgmma wait for the previous one.
 // NT == 0: that runtime loop, for conv_prog_kernel, whose wgmmas ptxas serializes for lack of registers anyway (C7512)
 // and where the unrolled groups only add spills.
-template <int BN, int MB, int NT>
+template <int BN, int MB, int NT, bool TF32>
 __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2], uint64_t (&adesc)[MB], uint64_t bdesc,
                                                uint32_t& accum, int& kx, int kw, uint32_t step_x, uint32_t step_row,
                                                uint32_t tap16) {
   using namespace ppx;
   if constexpr (NT == 0) {
     wgmma_fence();
-    for (int tt = 0; tt < tn; ++tt) halo_tap<BN, MB>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+    for (int tt = 0; tt < tn; ++tt) halo_tap<BN, MB, TF32>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
     wgmma_commit();
   } else {
     if constexpr (NT > 1) {
       if (tn < NT) {
-        halo_tap_group<BN, MB, NT - 1>(tn, acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+        halo_tap_group<BN, MB, NT - 1, TF32>(tn, acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
         return;
       }
     }
     wgmma_fence();
 #pragma unroll
-    for (int tt = 0; tt < NT; ++tt) halo_tap<BN, MB>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+    for (int tt = 0; tt < NT; ++tt) halo_tap<BN, MB, TF32>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
     wgmma_commit();
   }
 }
@@ -186,8 +194,8 @@ __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2],
 // Consumer side of one tile, run by each of the two consumer warpgroups: the main loop into register accumulators
 // (MB = h.MT m64 blocks of BN columns), then the epilogue of this warpgroup's pixel rows.  A stage is handed back to
 // its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
-// NT: see halo_tap_group.
-template <int BN, int MB, int NT>
+// NT: see halo_tap_group.  TF32: the split-tf32 form.
+template <int BN, int MB, int NT, bool TF32 = false>
 __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
                                           int wg, int t128) {
   using namespace ppx;
@@ -216,7 +224,7 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
     for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
       mbar_wait(&m.b_full[rb.s], rb.ph);
       const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(m.b + rb.s * m.b_stage_bytes));
-      halo_tap_group<BN, MB, NT>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+      halo_tap_group<BN, MB, NT, TF32>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
       wgmma_wait<1>();
       if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
       if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
@@ -265,7 +273,7 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
         };
         ppconv::epilogue_from_stage(p, src, mrow, t.g, n0 + cc, slot(0), slot(1));
       } else {
-        ppconv::epilogue_from_stage(p, src, mrow, t.g, n0 + cc, nullptr, nullptr);
+        ppconv::epilogue_from_stage<TF32>(p, src, mrow, t.g, n0 + cc, nullptr, nullptr);
       }
     });
   }
@@ -310,7 +318,7 @@ __device__ __forceinline__ void halo_produce_patches(const HaloParams& h, const 
       const int ci = c * 64;
       int q = 0;
 #pragma unroll
-      for (int k = 1; k < 4; ++k)
+      for (int k = 1; k < PP_MAX_SEGS; ++k)
         if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
       const int ch0 = t.g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
       mbar_wait(&m.a_empty[r.s], r.ph ^ 1);
@@ -349,7 +357,8 @@ __device__ __forceinline__ void halo_produce_weights(const HaloParams& h, const 
   }
 }
 
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_kernel(const __grid_constant__ HaloParams h) {
+template <bool TF32>
+__device__ __forceinline__ void halo_body(const HaloParams& h) {
   using namespace ppx;
   const HaloSmem m =
       halo_smem(halo_smem_base(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, h.tstore ? h.MT * h.out_stage_bytes : 0);
@@ -372,7 +381,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_kernel(const __grid_
     with_tile_shape(h.MT, h.c.BN, [&](auto bn, auto mb) {
       constexpr int BN = decltype(bn)::value;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
-        halo_tile<BN, decltype(mb)::value, halo_max_tps(BN)>(h, tile, m, ra, rb, stg, wg, t128);
+        halo_tile<BN, decltype(mb)::value, halo_max_tps(BN), TF32>(h, tile, m, ra, rb, stg, wg, t128);
     });
     if (h.tstore) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // outstanding stores of this thread complete
   } else if (warp == WARP_A) {
@@ -386,6 +395,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_kernel(const __grid_
       halo_produce_weights(h, m, r);
     }
   }
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_kernel(const __grid_constant__ HaloParams h) {
+  halo_body<false>(h);
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_tf32_kernel(const __grid_constant__ HaloParams h) {
+  halo_body<true>(h);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -582,6 +599,7 @@ int halo_num_sms(int* out) {
     PP_CUDA_CHECK(cudaGetDevice(&dev));
     PP_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_prog_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
   }
   *out = num_sms;
@@ -668,7 +686,7 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   // TMA-store epilogue (see HaloParams::tstore): flat layers with few K chunks, plain fp16 output
   h.tstore = 0;
   h.out_stage_bytes = 0;
-  if (!one_wave && flat && p.epi == PP_EPI_STD && !p.out_fp32 && p.groups == 1 && p.out_gstep == 0 && bn % 64 == 0 &&
+  if (!one_wave && flat && !p.split && p.epi == PP_EPI_STD && !p.out_fp32 && p.groups == 1 && p.out_gstep == 0 && bn % 64 == 0 &&
       p.vec_ok && h.chunks <= 16 && p.out_cstride % 8 == 0 && p.out_coff % 8 == 0 &&
       (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
     h.tstore = 1;
@@ -730,7 +748,7 @@ int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   int num_sms = 0;
   PP_TRY(halo_num_sms(&num_sms));
   const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, h.tstore ? h.MT * h.out_stage_bytes : 0).bytes;
-  return halo_launch(conv_halo_kernel, h, min(halo_total_tiles(h), num_sms), smem, stream);
+  return halo_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms), smem, stream);
 }
 
 // ---- multi-layer programs ------------------------------------------------------------------------------------------
@@ -763,6 +781,7 @@ int pp_prog_record_conv(const PPConvParams& p) {
   PP_REQUIRE(r != nullptr, "conv program: not recording");
   PP_REQUIRE(r->prog.n_layers < PROG_MAX_LAYERS, "conv program: more than %d layers", PROG_MAX_LAYERS);
   PP_REQUIRE(pp_conv_halo_eligible(p), "conv program: layer is not a stride-1 TMA halo-kernel convolution");
+  PP_REQUIRE(!p.split, "conv program: split-tf32 layers are not supported");
   const int li = r->prog.n_layers;
   PP_TRY(halo_configure(p, r->prog.layer[li], true));
   PP_REQUIRE(r->prog.layer[li].MT == 1 && r->prog.layer[li].c.BN <= 128, "conv program: layer tile %d x %d columns",

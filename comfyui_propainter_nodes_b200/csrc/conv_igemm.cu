@@ -7,6 +7,8 @@
 //                   streams the pre-swizzled weight tile with a single cp.async.bulk (TMA engine) per stage
 // Pipeline: `stages` smem slots (full/empty mbarriers) that keep filling across tile boundaries, so the producers run
 // ahead through the consumers' epilogue.
+// conv_igemm_tf32_kernel is the split-tf32 form (PPConvParams::split): the same body with tf32 MMAs (k8 per 32-byte
+// k-step instead of k16) and the split epilogue.
 #include <string.h>
 
 #include "conv_igemm.cuh"
@@ -23,7 +25,7 @@ constexpr int NUM_THREADS = 384;
 constexpr int MAX_STAGES = 8;
 constexpr int SMEM_BUDGET = 192 * 1024;
 
-template <int BN>
+template <int BN, bool TF32>
 __device__ __forceinline__ void igemm_consume(const PPConvParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
                                               uint64_t* empty_bar, float* stg, int wg, int t128) {
   using namespace ppx;
@@ -50,7 +52,10 @@ __device__ __forceinline__ void igemm_consume(const PPConvParams& p, uint8_t* sm
       const uint64_t adesc = gmma_desc_sw128_kmajor(a_addr + wg * (A_STAGE_BYTES / 2));
       const uint64_t bdesc = gmma_desc_sw128_kmajor(a_addr + A_STAGE_BYTES);
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) wgmma_f16<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kc | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < BK / 16; ++k) {
+        if constexpr (TF32) wgmma_tf32<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kc | k) != 0 ? 1u : 0u);
+        else wgmma_f16<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kc | k) != 0 ? 1u : 0u);
+      }
       wgmma_commit();
       wgmma_wait<1>();   // the previous chunk's MMAs are done: its slot may be refilled
       if (prev >= 0) mbar_arrive(&empty_bar[prev]);
@@ -63,12 +68,13 @@ __device__ __forceinline__ void igemm_consume(const PPConvParams& p, uint8_t* sm
     ppconv::drain_acc<BN>(acc, stg, t128, 4 + wg, [&](const float* src, int r, int c) {
       const int m = m0 + wg * 64 + r;
       if (m < p.M_total && n0 + c < p.Cout_g)
-        ppconv::epilogue_from_stage(p, src, m, g, n0 + c, nullptr, nullptr);
+        ppconv::epilogue_from_stage<TF32>(p, src, m, g, n0 + c, nullptr, nullptr);
     });
   }
 }
 
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid_constant__ PPConvParams p) {
+template <bool TF32>
+__device__ __forceinline__ void igemm_body(const PPConvParams& p) {
   using namespace ppx;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -106,7 +112,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
     setmaxnreg_inc<216>();
     const int wg = tid >> 7;
     ppconv::with_tile_width<256>(p.BN, [&](auto bn) {
-      igemm_consume<decltype(bn)::value>(p, smem, stage_bytes, full_bar, empty_bar, stg + wg * (ppconv::STG_BYTES / 4), wg,
+      igemm_consume<decltype(bn)::value, TF32>(p, smem, stage_bytes, full_bar, empty_bar, stg + wg * (ppconv::STG_BYTES / 4), wg,
                                          tid & 127);
     });
   } else {
@@ -158,7 +164,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
         const bool kvalid = k < p.K_total;
         int q = 0;
 #pragma unroll
-        for (int t = 1; t < 4; ++t)
+        for (int t = 1; t < PP_MAX_SEGS; ++t)
           if (t < p.nseg && ci >= p.seg[t].cbegin) q = t;
         const __half* sbase = p.seg[q].ptr + p.seg[q].coff + g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
         const long long cs = p.seg[q].cstride;
@@ -192,6 +198,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid
   }
 }
 
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_kernel(const __grid_constant__ PPConvParams p) {
+  igemm_body<false>(p);
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_tf32_kernel(const __grid_constant__ PPConvParams p) {
+  igemm_body<true>(p);
+}
+
 }  // namespace
 
 namespace {
@@ -204,7 +218,7 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   PP_REQUIRE(p.BN >= 16 && p.BN <= 256 && p.BN % 16 == 0, "conv: BN=%d must be a multiple of 16 in [16,256]", p.BN);
   PP_REQUIRE(p.Cout_g_pad % p.BN == 0, "conv: Cout_g_pad=%d not a multiple of BN=%d", p.Cout_g_pad, p.BN);
   PP_REQUIRE(p.Cin % 8 == 0, "conv: Cin=%d must be a multiple of 8", p.Cin);
-  PP_REQUIRE(p.nseg >= 1 && p.nseg <= 4, "conv: nseg=%d", p.nseg);
+  PP_REQUIRE(p.nseg >= 1 && p.nseg <= PP_MAX_SEGS, "conv: nseg=%d", p.nseg);
   PP_REQUIRE(p.seg[p.nseg - 1].cend == p.Cin && p.seg[0].cbegin == 0, "conv: segments do not cover Cin=%d", p.Cin);
   for (int i = 0; i < p.nseg; ++i) {
     PP_REQUIRE(p.seg[i].cstride % 8 == 0 && p.seg[i].coff % 8 == 0 && p.seg[i].gstep % 8 == 0 &&
@@ -217,7 +231,18 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   p.num_kc = pp_ceil_div(p.K_total, BK);
   p.M_total = p.N * p.OH * p.OW;
   if (p.M_total <= 0) return PP_OK;
-  {
+  if (p.split) {
+    // every epilogue tensor is fp32: 16-byte runs need 4-float aligned pointers, strides, offsets and hi -> lo distances
+    auto al = [](const void* ptr, long long cs, long long co, long long gs, long long lo) {
+      return ptr == nullptr || ((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cs % 4 == 0 && co % 4 == 0 && gs % 4 == 0 &&
+                                lo % 4 == 0);
+    };
+    bool ok = al(p.out, p.out_cstride, p.out_coff, p.out_gstep, p.out_fp32 ? 0 : p.out_lo) &&
+              al(p.aux0, p.aux0_cstride, p.aux0_coff, 0, p.aux0_lo) && al(p.aux1, p.aux1_cstride, p.aux1_coff, 0, p.aux1_lo) &&
+              al(p.out2, p.out2_cstride, p.out2_coff, 0, p.out2_lo);
+    if (p.epi == PP_EPI_GRU_ZR) ok = ok && ((p.Cout_g >> 1) % 16 == 0);
+    p.vec_ok = ok ? 1 : 0;
+  } else {
     const int esz = p.out_fp32 ? 4 : 2, per16 = 16 / esz;
     auto al = [](const void* ptr, long long cs, long long co, long long gs, int per) {
       return ptr == nullptr || ((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cs % per == 0 && co % per == 0 && gs % per == 0);
@@ -228,7 +253,11 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
     if (p.epi == PP_EPI_GRU_ZR) ok = ok && ((p.Cout_g >> 1) % 16 == 0);
     p.vec_ok = ok ? 1 : 0;
   }
-  if (pp_prog_recording()) { g_last_kind = 'p'; return pp_prog_record_conv(p); }
+  if (pp_prog_recording()) {
+    PP_REQUIRE(!p.split, "conv program: split-tf32 layers are not supported");
+    g_last_kind = 'p';
+    return pp_prog_record_conv(p);
+  }
   if (pp_conv_halo_eligible(p)) { g_last_kind = 'h'; return pp_launch_conv_halo(p, stream); }
   g_last_kind = 'i';
   for (int i = 0; i < p.nseg; ++i)
@@ -245,6 +274,7 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
     PP_CUDA_CHECK(cudaGetDevice(&dev));
     PP_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_igemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   }
   const long long total_tiles = (long long)pp_ceil_div(p.M_total, BM) * (p.Cout_g_pad / p.BN) * p.groups;
   PP_REQUIRE(total_tiles < (1LL << 31), "conv: too many tiles");
@@ -260,7 +290,7 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_igemm_kernel, p));
+  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, p.split ? conv_igemm_tf32_kernel : conv_igemm_kernel, p));
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }

@@ -5,7 +5,14 @@
 //
 // Activations are NHWC fp16 with channel strides that are multiples of 8 (16 B), so every 16-byte
 // im2col vector lies inside one filter tap.  A conv input may be the channel-concatenation of up to
-// four tensors (segments): the torch.cat calls of the reference become address arithmetic here.
+// PP_MAX_SEGS tensors (segments): the torch.cat calls of the reference become address arithmetic here.
+//
+// Split-tf32 form (PPConvParams::split = 1, the fp32 RAFT path): every activation tensor is fp32 and stores each
+// channel as a pair hi = tf32(x), lo = x - hi, the hi values of the C channels of a pixel followed by the lo values
+// ([pix][hi C | lo C], hi + lo == x exactly).  A conv reads the segments (hi, lo, hi) against a weight image whose K rows
+// are [W_hi; W_hi; W_lo], so one tf32 GEMM computes hi*W_hi + lo*W_hi + hi*W_lo ~ x*W to ~2^-21 (3xTF32).  The
+// producers only move bytes: segment fields, Cin and the weight image are given in 2-byte units (a 128-byte K-chunk row
+// holds 32 fp32 values instead of 64 fp16), and only the MMA instruction and the epilogue differ.
 #pragma once
 #include "pp_common.cuh"
 
@@ -29,8 +36,10 @@ struct PPConvSeg {
                  // zero (TMA out-of-bounds fill; halo kernel only) -- lets a 32-channel tensor feed 64-wide K chunks
 };
 
+constexpr int PP_MAX_SEGS = 6;   // gru.q of the split-tf32 path: (r*h, x) x (hi, lo, hi)
+
 struct PPConvParams {
-  PPConvSeg seg[4];
+  PPConvSeg seg[PP_MAX_SEGS];
   int nseg;
   int N, H, W, OH, OW;
   int Cin;                // per-group input channels as seen by the kernel (multiple of 8)
@@ -51,6 +60,10 @@ struct PPConvParams {
   const __half* aux0; int aux0_cstride, aux0_coff;   // residual (STD) or h (GRU)
   const __half* aux1; int aux1_cstride, aux1_coff;   // z (GRU_H)
   __half* out2; int out2_cstride, out2_coff;          // r*h destination (GRU_ZR)
+  // split-tf32 form (see above): 1 = tf32 MMAs; out / aux0 / aux1 / out2 are fp32 [hi | lo] tensors whose lo value of a
+  // channel lies *_lo floats after its hi value (strides and offsets in floats).  out_fp32 = 1 writes plain fp32 instead.
+  int split;
+  int out_lo, aux0_lo, aux1_lo, out2_lo;
 };
 
 int pp_launch_conv(const PPConvParams& p, cudaStream_t stream);

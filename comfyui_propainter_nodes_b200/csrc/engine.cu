@@ -42,7 +42,7 @@ PPConvCall::PPConvCall(PPEngine& e, const std::string& name_, int N, int H, int 
 
 PPConvCall& PPConvCall::in(const __half* ptr, int cs, int co, int channels, int gstep) {
   if (err != PP_OK) return *this;
-  if (p.nseg >= 4) { pp_set_error("conv: more than 4 input segments"); err = PP_ERR_ARG; return *this; }
+  if (p.nseg >= PP_MAX_SEGS) { pp_set_error("conv: more than %d input segments", PP_MAX_SEGS); err = PP_ERR_ARG; return *this; }
   PPConvSeg& s = p.seg[p.nseg];
   s.ptr = ptr; s.cstride = cs; s.coff = co; s.gstep = gstep;
   s.cbegin = p.nseg == 0 ? 0 : p.seg[p.nseg - 1].cend;
@@ -85,9 +85,58 @@ PPConvCall& PPConvCall::gru_h(const __half* h, int h_cs, int h_co, const __half*
   return *this;
 }
 
+PPConvCall& PPConvCall::tf32() {
+  p.split = 1;
+  return *this;
+}
+
+PPConvCall& PPConvCall::in_split(const float* ptr, int C, int co, int channels) {
+  if (err != PP_OK) return *this;
+  if (!p.split || n_split_in >= PP_MAX_SEGS / 3) {
+    pp_set_error("conv %s: in_split needs tf32() and at most %d inputs", name.c_str(), PP_MAX_SEGS / 3);
+    err = PP_ERR_ARG;
+    return *this;
+  }
+  split_in[n_split_in++] = SplitIn{ptr, C, co, channels};
+  return *this;
+}
+
+PPConvCall& PPConvCall::out_split(float* ptr, int C, int co) {
+  p.out = ptr; p.out_cstride = 2 * C; p.out_coff = co; p.out_lo = C; p.out_fp32 = 0; p.out_gstep = 0;
+  return *this;
+}
+
+PPConvCall& PPConvCall::residual_split(const float* ptr, int C, int co) {
+  p.aux0 = reinterpret_cast<const __half*>(ptr); p.aux0_cstride = 2 * C; p.aux0_coff = co; p.aux0_lo = C;
+  return *this;
+}
+
+PPConvCall& PPConvCall::gru_zr_split(const float* h, int h_C, int h_co, float* rh, int rh_C, int rh_co) {
+  p.epi = PP_EPI_GRU_ZR;
+  p.aux0 = reinterpret_cast<const __half*>(h); p.aux0_cstride = 2 * h_C; p.aux0_coff = h_co; p.aux0_lo = h_C;
+  p.out2 = reinterpret_cast<__half*>(rh); p.out2_cstride = 2 * rh_C; p.out2_coff = rh_co; p.out2_lo = rh_C;
+  return *this;
+}
+
+PPConvCall& PPConvCall::gru_h_split(const float* h, int h_C, int h_co, const float* z, int z_C, int z_co) {
+  p.epi = PP_EPI_GRU_H;
+  p.aux0 = reinterpret_cast<const __half*>(h); p.aux0_cstride = 2 * h_C; p.aux0_coff = h_co; p.aux0_lo = h_C;
+  p.aux1 = reinterpret_cast<const __half*>(z); p.aux1_cstride = 2 * z_C; p.aux1_coff = z_co; p.aux1_lo = z_C;
+  return *this;
+}
+
 int PPConvCall::run(cudaStream_t st) {
   if (err != PP_OK) return err;
-  if (p.nseg > 0 && p.seg[p.nseg - 1].cend < p.Cin && p.Cin % 64 == 0 && p.Cin - p.seg[p.nseg - 1].cend < 64 &&
+  if (p.split) {
+    // (hi, lo, hi) passes over the inputs, in the kernel's 2-byte units: an fp32 channel is two of them
+    PP_REQUIRE(p.nseg == 0 && n_split_in > 0, "conv %s: split-tf32 inputs must all come from in_split", name.c_str());
+    for (int pass = 0; pass < 3; ++pass)
+      for (int i = 0; i < n_split_in; ++i) {
+        const SplitIn& s = split_in[i];
+        in(reinterpret_cast<const __half*>(s.ptr), 4 * s.C, 2 * (s.co + (pass == 1 ? s.C : 0)), 2 * s.channels);
+      }
+    if (err != PP_OK) return err;
+  } else if (p.nseg > 0 && p.seg[p.nseg - 1].cend < p.Cin && p.Cin % 64 == 0 && p.Cin - p.seg[p.nseg - 1].cend < 64 &&
       p.seg[p.nseg - 1].gstep == 0) {
     // weights registered with their input channels zero-padded to a 64 multiple (engine.py PAD64_CONVS): the last
     // segment's tensor only holds `cvalid` channels, the TMA loads of the halo kernel zero-fill the rest

@@ -122,7 +122,21 @@ struct PPConvCall {
   PPConvCall& residual(const __half* ptr, int cs, int co);
   PPConvCall& gru_zr(const __half* h, int h_cs, int h_co, __half* rh, int rh_cs, int rh_co);
   PPConvCall& gru_h(const __half* h, int h_cs, int h_co, const __half* z, int z_cs, int z_co);
+  // Split-tf32 form (PPConvParams::split, conv_igemm.cuh): the weights must have been registered as a split image.  Every
+  // tensor is an fp32 [pix][hi C | lo C] pair tensor given by its pointer and real channel count C; `co` / `channels` count
+  // fp32 channels.  The input segments added with in_split are read as (hi..., lo..., hi...) by run().
+  PPConvCall& tf32();
+  PPConvCall& in_split(const float* ptr, int C, int co, int channels);
+  PPConvCall& out_split(float* ptr, int C, int co);
+  PPConvCall& residual_split(const float* ptr, int C, int co);
+  PPConvCall& gru_zr_split(const float* h, int h_C, int h_co, float* rh, int rh_C, int rh_co);
+  PPConvCall& gru_h_split(const float* h, int h_C, int h_co, const float* z, int z_C, int z_co);
   int run(cudaStream_t st);
+
+ private:
+  struct SplitIn { const float* ptr; int C, co, channels; };
+  SplitIn split_in[PP_MAX_SEGS / 3];
+  int n_split_in = 0;
 };
 
 void pp_build_ring_indices(int nh, int nw, std::vector<int>& out);
@@ -135,8 +149,9 @@ int pp_comm_all_gather_blocks_impl(PPEngine& e, void* buf, const long long* row_
                                    size_t row_bytes, int first_rank, int n_members, cudaStream_t st);
 
 // ---- stages ---------------------------------------------------------------------------------------
+// fp32: the split-tf32 path (weights registered under "<name>.tf32", see engine.py); otherwise fp16 activations
 int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
-                  cudaStream_t st);
+                  bool fp32, cudaStream_t st);
 int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
                            int H, int W, float* out_f, float* out_b, int team_first, int team_size, cudaStream_t st);
 int pp_stage_image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f,

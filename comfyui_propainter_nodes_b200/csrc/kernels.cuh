@@ -36,6 +36,22 @@ int pp_k_raft_coords_update(const float* delta, float* coords1, __half* flow8, _
 int pp_k_flow_patch7x7(const __half* flow8, __half* out /*[M][128]*/, int B, int h8, int w8, cudaStream_t st);
 int pp_k_convex_upsample(const float* coords1, const __half* mask, float* out_nchw, int B, int h8, int w8,
                          cudaStream_t st);
+// fp32 RAFT path: split-tf32 pair tensors [pix][hi C | lo C] (conv_igemm.cuh), fp32 correlation pyramid
+int pp_k_nchw_f32_to_split(const float* src, float* dst, int N, int C, int H, int W, int cs, cudaStream_t st);
+int pp_k_instnorm_stats_f32(const float* x, int N, int HW, int C, float* sums, cudaStream_t st);
+int pp_k_instnorm_apply_f32(const float* x, const float* sums, const float* residual, float* out, int N, int HW, int C,
+                            int relu, cudaStream_t st);
+int pp_k_pack_b_operand_split(const float* src, float* dst, int G, int R, int R_pad, int K, cudaStream_t st);
+int pp_k_corr_pool_f32(const float* src, float* dst, long long nq, int h, int w, cudaStream_t st);
+int pp_k_corr_lookup_f32(const float* l0, const float* l1, const float* l2, const float* l3, const float* coords,
+                         float* out /*[nq][hi out_C | lo out_C]*/, int out_C, long long nq, int h8, int w8, cudaStream_t st);
+int pp_k_cnet_split_f32(const float* c, float* hx, int hx_C, long long npix, cudaStream_t st);
+// delta == nullptr: coords1 = coords0 (init)
+int pp_k_raft_coords_f32(const float* delta, float* coords1, float* hx, int hx_C, int hx_flow_co, int B, int h8, int w8,
+                         cudaStream_t st);
+int pp_k_flow_patch7x7_f32(const float* coords1, float* out /*[M][hi 128 | lo 128]*/, int B, int h8, int w8, cudaStream_t st);
+int pp_k_convex_upsample_f32(const float* coords1, const float* mask, float* out_nchw, int B, int h8, int w8,
+                             cudaStream_t st);
 
 // ---- propagation (kernels_prop.cu) --------------------------------------------------------------
 int pp_k_imgprop_step(const __half* cur, const __half* prop_in, __half* prop_out, const __half* flow_prop,

@@ -39,6 +39,7 @@ _SIGNATURES = {
     "pp_register_tensor": (_I, [_VP, _CP, _VP, _SZ]),
     "pp_set_conv_macs": (_I, [_VP, _CP, ctypes.c_double]),
     "pp_raft_bidir": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP]),
+    "pp_raft_bidir_fp32": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP]),
     "pp_flow_complete": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
     "pp_flow_complete_dist": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _I, _I, _VP]),
     "pp_image_propagate": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
@@ -137,6 +138,47 @@ def pack_conv_weight(w: torch.Tensor, groups: int = 1, cin_map=None):
     buf = torch.gather(buf, 3, pos.view(1, 1, cout_g_pad, 8, 1).expand(groups, num_kc, cout_g_pad, 8, 8))
     meta = dict(cout_g=cout_g, cout_g_pad=cout_g_pad, bn=bn, cin_g=cin_k, kh=kh, kw=kw, groups=groups)
     return buf.to(torch.float16).contiguous(), meta
+
+
+def split_tf32(x: torch.Tensor):
+    """fp32 x -> (hi, lo): hi = x rounded to tf32 (10 explicit mantissa bits, nearest, ties away from zero, as
+    cvt.rna.tf32.f32 does), lo = x - hi.  hi has its low 13 mantissa bits zero and hi + lo == x exactly."""
+    x = x.detach().float().contiguous()
+    hi = ((x.view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
+    return hi, x - hi
+
+
+def pack_conv_weight_tf32(w, cin_map=None):
+    """[Cout, Cin, kh, kw] fp32 -> split-tf32 B-operand image of the fp32 RAFT path + metadata.
+
+    The kernel reads its inputs as the segments (hi, lo, hi) of split activation pairs (csrc/conv_igemm.cuh), so the K
+    rows of one filter tap are [W_hi; W_hi; W_lo] over the kernel's input channels (``cin_map`` as in
+    pack_conv_weight, padded to a multiple of 4 channels), and the GEMM sums hi*W_hi + lo*W_hi + hi*W_lo.  K is
+    ordered (ky, kx, pass, ci).  Layout: [K_pad/32][cout_pad] rows of 32 fp32 (128 bytes, the same byte geometry as the
+    fp16 image); inside a row the 16-byte unit u is stored at position u ^ (row & 7).  ``cin_g`` of the metadata counts
+    the kernel's 2-byte units (two per fp32 value)."""
+    w = w.detach().float().cpu()
+    cout, cin_ref, kh, kw = w.shape
+    if cin_map is None:
+        cin_map = list(range(cin_ref)) + [-1] * ((-cin_ref) % 4)
+    assert len(cin_map) % 4 == 0
+    cin_k = len(cin_map)
+    idx = torch.tensor([max(i, 0) for i in cin_map], dtype=torch.long)
+    keep = torch.tensor([1.0 if i >= 0 else 0.0 for i in cin_map])
+    hi, lo = split_tf32(w[:, idx] * keep.view(1, -1, 1, 1))               # [Cout, cin_k, kh, kw]
+    wk = torch.cat([hi, hi, lo], 1).permute(0, 2, 3, 1).reshape(cout, kh * kw * 3 * cin_k)
+    bn, cout_pad = choose_bn(cout)
+    K = wk.shape[1]
+    K_pad = (K + 31) // 32 * 32
+    buf = torch.zeros(cout_pad, K_pad)
+    buf[:cout, :K] = wk
+    num_kc = K_pad // 32
+    buf = buf.view(cout_pad, num_kc, 8, 4).permute(1, 0, 2, 3).contiguous()           # [kc, row, unit, 4]
+    rows = torch.arange(cout_pad)
+    pos = torch.arange(8).view(1, 8) ^ (rows.view(-1, 1) & 7)                          # position p holds unit p^(r&7)
+    buf = torch.gather(buf, 2, pos.view(1, cout_pad, 8, 1).expand(num_kc, cout_pad, 8, 4))
+    meta = dict(cout_g=cout, cout_g_pad=cout_pad, bn=bn, cin_g=2 * 3 * cin_k, kh=kh, kw=kw, groups=1)
+    return buf.contiguous(), meta
 
 
 def _fold_bn(w, b, sd, p, eps=1e-5):
@@ -387,6 +429,18 @@ class Engine:
                                               meta["groups"]))
         self._check(self.lib.pp_set_conv_macs(self.h, name.encode(), float(w.numel() if macs is None else macs)))
 
+    def register_conv_tf32(self, name, w, b, cin_map=None, macs=None):
+        """Split-tf32 image of a layer (pack_conv_weight_tf32), registered as ``name + ".tf32"``."""
+        packed, meta = pack_conv_weight_tf32(w, cin_map)
+        packed = packed.to(self.device)
+        bias = None if b is None else b.detach().float().contiguous().to(self.device)
+        self._keep += [packed, bias]
+        self.conv_meta[name + ".tf32"] = meta
+        self._check(self.lib.pp_register_conv(self.h, (name + ".tf32").encode(), _ptr(packed), _ptr(bias), meta["cout_g"],
+                                              meta["cout_g_pad"], meta["bn"], meta["cin_g"], meta["kh"], meta["kw"], 1))
+        self._check(self.lib.pp_set_conv_macs(self.h, (name + ".tf32").encode(),
+                                              float(w.numel() if macs is None else macs)))
+
     def register_tensor(self, name, t):
         t = t.detach().float().contiguous().to(self.device)
         self._keep.append(t)
@@ -401,9 +455,16 @@ class Engine:
         "gen.fp.backward_1.offset.0", "gen.fp.forward_1.offset.0", "gen.fp.backward_1.backbone.0",
         "gen.fp.forward_1.backbone.0", "gen.fp.fuse.0")
 
+    # fp32 RAFT path: kernel input channels of the split images whose reference channels are not a multiple of 32
+    # (the frames: 3 -> 4, one 16-byte vector; the correlation lookup: 324 -> 352, whole 32-channel K chunks per pass)
+    TF32_CIN_MAPS = {"raft.fnet.conv1": (3, 4), "raft.cnet.conv1": (3, 4), "raft.update.convc1": (324, 352)}
+
     def load_weights(self, raft_sd, rfc_sd, gen_sd):
         convs, tens = build_layers(raft_sd, rfc_sd, gen_sd)
         for name, (w, b, groups, cin_map, macs) in convs.items():
+            if name.startswith("raft."):
+                tm = self.TF32_CIN_MAPS.get(name)
+                self.register_conv_tf32(name, w, b, None if tm is None else _pad_map(*tm), macs)
             if name in self.PAD64_CONVS:
                 cin_map = list(cin_map) if cin_map is not None else list(range(w.shape[1]))
                 cin_map += [-1] * ((-len(cin_map)) % 64)
@@ -416,9 +477,11 @@ class Engine:
     def _f32(self, t):
         return t.to(device=self.device, dtype=torch.float32).contiguous()
 
-    def raft_bidir(self, frames: torch.Tensor, iters: int, out=None):
+    def raft_bidir(self, frames: torch.Tensor, iters: int, out=None, fp32: bool = False):
         """frames [T,3,H,W] in [-1,1] -> (flows_f, flows_b) [T-1,2,H,W] (written into `out` when given: contiguous
-        float32 views, e.g. a rank's shard of the full flow buffers)."""
+        float32 views, e.g. a rank's shard of the full flow buffers).  fp32=False: fp16 activations with fp32
+        accumulation; fp32=True: fp32 activations and 3xTF32 GEMMs (pp_raft_bidir_fp32), what the node runs for
+        fp16="disable"."""
         frames = self._f32(frames)
         T, _, H, W = frames.shape
         if out is not None:
@@ -427,7 +490,8 @@ class Engine:
         else:
             ff = torch.empty(T - 1, 2, H, W, device=self.device, dtype=torch.float32)
             fb = torch.empty_like(ff)
-        self._check(self.lib.pp_raft_bidir(self.h, _ptr(frames), T, H, W, int(iters), _ptr(ff), _ptr(fb), self._stream()))
+        fn = self.lib.pp_raft_bidir_fp32 if fp32 else self.lib.pp_raft_bidir
+        self._check(fn(self.h, _ptr(frames), T, H, W, int(iters), _ptr(ff), _ptr(fb), self._stream()))
         return ff, fb
 
     def flow_complete(self, flows_f, flows_b, flow_masks):

@@ -159,7 +159,7 @@ def inpaint_clip_distributed(models, frames, flow_masks, masks_dilated, orig_u8,
     ff = torch.empty(n_pairs, 2, H, W, device=dev, dtype=torch.float32)
     fb = torch.empty_like(ff)
     if hi > lo:
-        eng.raft_bidir(frames[0, lo:hi + 1], cfg.raft_iter, out=(ff[lo:hi], fb[lo:hi]))
+        eng.raft_bidir(frames[0, lo:hi + 1], cfg.raft_iter, out=(ff[lo:hi], fb[lo:hi]), fp32=not cfg.use_half)
     mark("raft")
     sizes = shard_sizes(n_pairs, world)
     gather_rows(eng, ff, sizes, 0, group)

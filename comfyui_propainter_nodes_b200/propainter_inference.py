@@ -10,8 +10,10 @@ exactly where the reference calls its PyTorch modules:
 * image_propagation   -> Engine.image_propagate   (:159-225, chunks of min(100, subvideo_length) with a 10-frame halo)
 * feature_propagation -> Engine.gen_begin/gen_window/composite (:228-311)
 
-Tensors keep the reference layouts ([1,T,C,H,W]); the engine computes in fp16 with fp32 accumulation
-regardless of the ``fp16`` switch (the switch only selects the dtype of the tensors handed back).
+Tensors keep the reference layouts ([1,T,C,H,W]).  RAFT follows the ``fp16`` switch: "enable" runs it with fp16
+activations and fp32 accumulation, "disable" at fp32 accuracy (fp32 activations, 3xTF32 GEMMs), like the reference,
+which always runs RAFT in fp32.  Flow completion and the generator compute in fp16 with fp32 accumulation in both
+modes (there the switch only selects the dtype of the tensors handed back).
 """
 from __future__ import annotations
 
@@ -65,7 +67,7 @@ def compute_flow(raft_model, frames: torch.Tensor, config: ProPainterConfig):
     The reference splits the clip into <=12/8/4/2-frame pieces only to bound memory; pairs are independent,
     so the engine batches all of them (it chunks internally against its workspace)."""
     eng = raft_model.engine
-    ff, fb = eng.raft_bidir(frames[0], config.raft_iter)
+    ff, fb = eng.raft_bidir(frames[0], config.raft_iter, fp32=not config.use_half)
     return ff.unsqueeze(0), fb.unsqueeze(0)
 
 

@@ -5,7 +5,7 @@
  * boundary.  Tensors are contiguous, float32, in the layouts the reference's own tensors have at the same
  * call sites (paths relative to daniabib/ComfyUI_ProPainter_Nodes):
  *
- *   pp_raft_bidir          replaces  raft_model(frames, iters)                propainter_inference.py:77-93
+ *   pp_raft_bidir[_fp32]   replaces  raft_model(frames, iters)                propainter_inference.py:77-93
  *                                    (RAFT_bi.forward, model/modules/flow_comp_raft.py:39-58)
  *   pp_flow_complete       replaces  forward_bidirect_flow + combine_flow     propainter_inference.py:123-150
  *                                    (model/recurrent_flow_completion.py:356-400)
@@ -69,9 +69,14 @@ PP_API int pp_comm_destroy(pp_handle h);
 PP_API int pp_comm_all_gather_rows(pp_handle h, void* buf, const long long* rows_per_member, size_t row_bytes,
                                    int first_rank, int n_members, void* stream);
 
-/* frames [T,3,H,W] in [-1,1]  ->  flows_f, flows_b [T-1,2,H,W]. */
+/* frames [T,3,H,W] in [-1,1]  ->  flows_f, flows_b [T-1,2,H,W].  fp16 activations, fp32 accumulation. */
 PP_API int pp_raft_bidir(pp_handle h, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
                   void* stream);
+/* The same at fp32 accuracy (the node's fp16="disable"): fp32 activations, every convolution and the correlation as
+ * error-compensated tf32 GEMMs (3xTF32), fp32 correlation pyramid.  Needs the RAFT weights also registered as split
+ * images under "<name>.tf32" (engine.py registers both). */
+PP_API int pp_raft_bidir_fp32(pp_handle h, const float* frames, int T, int H, int W, int iters, float* flows_f,
+                              float* flows_b, void* stream);
 /* flows [T-1,2,H,W], flow_masks [T,1,H,W]  ->  completed flows [T-1,2,H,W] (prediction inside the mask). */
 PP_API int pp_flow_complete(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T, int H,
                      int W, float* out_f, float* out_b, void* stream);
