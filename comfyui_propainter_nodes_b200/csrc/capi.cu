@@ -420,6 +420,87 @@ int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l
                           static_cast<__half*>(out_f16), 328, nq, h8 * w8, h8, w8, as_stream(stream));
 }
 
+int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, int x0_co, int x0_ch, const float* x1,
+                    int x1_C, int x1_co, int x1_ch, int N, int H, int W, int sh, int sw, int ph, int pw, int epi, int act,
+                    float slope, float scale, int act2, const float* aux0, int aux0_C, int aux0_co, float* aux1,
+                    int aux1_C, int aux1_co, float* out, int out_C, int out_co, int out_fp32, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(name && x0 && out, "pp_op_conv_tf32: null pointer");
+  PP_REQUIRE(epi == PP_EPI_STD || (aux0 && aux1), "pp_op_conv_tf32: the GRU epilogues need aux0 and aux1");
+  PPConvCall c(e, name, N, H, W);
+  c.tf32().in_split(x0, x0_C, x0_co, x0_ch);
+  if (x1 != nullptr) c.in_split(x1, x1_C, x1_co, x1_ch);
+  c.geom(sh, sw, ph, pw);
+  if (out_fp32) c.out(out, out_C, out_co, 1);
+  else c.out_split(out, out_C, out_co);
+  if (epi == PP_EPI_GRU_ZR) {
+    c.gru_zr_split(aux0, aux0_C, aux0_co, aux1, aux1_C, aux1_co);
+  } else if (epi == PP_EPI_GRU_H) {
+    c.gru_h_split(aux0, aux0_C, aux0_co, aux1, aux1_C, aux1_co);
+  } else {
+    c.act(act, slope, scale, act2);
+    if (aux0 != nullptr) c.residual_split(aux0, aux0_C, aux0_co);
+  }
+  return c.run(as_stream(stream));
+}
+
+int pp_op_instnorm(pp_handle h, const void* x, const void* residual, void* out, int N, int HW, int C, int relu, int fp32,
+                   void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(x && out, "pp_op_instnorm: null pointer");
+  ArenaGuard guard(e.arena);
+  float* sums;
+  PP_TRY(pp_alloc(e, &sums, pp_k_instnorm_scratch_floats(N, HW, C), "instnorm sums"));
+  cudaStream_t st = as_stream(stream);
+  if (fp32) {
+    PP_TRY(pp_k_instnorm_stats_f32(static_cast<const float*>(x), N, HW, C, sums, st));
+    PP_TRY(pp_k_instnorm_apply_f32(static_cast<const float*>(x), sums, static_cast<const float*>(residual),
+                                   static_cast<float*>(out), N, HW, C, relu, st));
+  } else {
+    PP_TRY(pp_k_instnorm_stats(static_cast<const __half*>(x), N, HW, C, sums, st));
+    PP_TRY(pp_k_instnorm_apply(static_cast<const __half*>(x), sums, static_cast<const __half*>(residual),
+                               static_cast<__half*>(out), N, HW, C, relu, st));
+  }
+  PP_CUDA_CHECK(cudaStreamSynchronize(st));   // the scratch goes back to the arena on return
+  return PP_OK;
+}
+
+int pp_op_corr_pyramid(pp_handle h, const void* fmap1, const void* fmap2, int pairs, int h8, int w8, int fp32, void* l0,
+                       void* l1, void* l2, void* l3, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(fmap1 && fmap2 && l0 && l1 && l2 && l3 && pairs >= 1, "pp_op_corr_pyramid: bad argument");
+  ArenaGuard guard(e.arena);
+  cudaStream_t st = as_stream(stream);
+  const int P = h8 * w8, P_pad = pp_raft_corr_pad(P);
+  uint8_t* fpack;
+  PP_TRY(pp_alloc(e, &fpack, (size_t)pairs * P_pad * 256 * (fp32 ? 12 : 2), "fmap packed"));
+  if (fp32) PP_TRY(pp_k_pack_b_operand_split(static_cast<const float*>(fmap2), reinterpret_cast<float*>(fpack), pairs, P,
+                                             P_pad, 256, st));
+  else PP_TRY(pp_k_pack_b_operand(static_cast<const __half*>(fmap2), reinterpret_cast<__half*>(fpack), pairs, P, P_pad,
+                                  256, st));
+  e.launches++;
+  PP_TRY(pp_raft_corr_volume(e, fmap1, fpack, pairs, P, P_pad, fp32 != 0, l0, st));
+  void* const corr[4] = {l0, l1, l2, l3};
+  PP_TRY(pp_raft_corr_pool(e, corr, (long long)pairs * P, h8, w8, fp32 != 0, st));
+  PP_CUDA_CHECK(cudaStreamSynchronize(st));
+  return PP_OK;
+}
+
+int pp_op_corr_lookup_f32(pp_handle h, const float* l0, const float* l1, const float* l2, const float* l3,
+                          const float* coords, float* out, long long nq, int h8, int w8, void* stream) {
+  PP_HANDLE(h);
+  e.launches++;
+  return pp_k_corr_lookup_f32(l0, l1, l2, l3, coords, out, 352, nq, h8, w8, as_stream(stream));
+}
+
+int pp_op_convex_upsample(pp_handle h, const float* coords1, const void* mask, float* out, int B, int h8, int w8, int fp32,
+                          void* stream) {
+  PP_HANDLE(h);
+  e.launches++;
+  if (fp32) return pp_k_convex_upsample_f32(coords1, static_cast<const float*>(mask), out, B, h8, w8, as_stream(stream));
+  return pp_k_convex_upsample(coords1, static_cast<const __half*>(mask), out, B, h8, w8, as_stream(stream));
+}
+
 int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* prop_in4_f16, void* prop_out4_f16,
                        const void* flow_prop_f16, const void* flow_check_f16, int H, int W, void* stream) {
   PP_HANDLE(h);

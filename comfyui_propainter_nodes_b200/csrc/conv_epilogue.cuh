@@ -6,25 +6,28 @@
 
 namespace ppconv {
 
-template <int ACT>
+// ACC (the split-tf32 epilogue): fp32-accurate tanh (pp_common.cuh) instead of the fast-math tanh.approx, whose error is
+// below the fp16 storage rounding but far above fp32's
+template <int ACT, bool ACC = false>
 __device__ __forceinline__ void act16_t(float (&v)[16], float slope) {
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
     if (ACT == PP_ACT_RELU) v[i] = fmaxf(v[i], 0.f);
     else if (ACT == PP_ACT_LRELU) v[i] = v[i] > 0.f ? v[i] : v[i] * slope;
     else if (ACT == PP_ACT_SIGMOID) v[i] = ppx::sigmoidf_(v[i]);
-    else if (ACT == PP_ACT_TANH) v[i] = tanhf(v[i]);
+    else if (ACT == PP_ACT_TANH) v[i] = ACC ? ppx::tanh_acc(v[i]) : tanhf(v[i]);
     else if (ACT == PP_ACT_GELU) v[i] = ppx::gelu_erf(v[i]);
   }
 }
 // one (uniform) branch per 16 values instead of one per value
+template <bool ACC = false>
 __device__ __forceinline__ void act16(float (&v)[16], int act, float slope) {
   switch (act) {
-    case PP_ACT_RELU: act16_t<PP_ACT_RELU>(v, slope); break;
-    case PP_ACT_LRELU: act16_t<PP_ACT_LRELU>(v, slope); break;
-    case PP_ACT_SIGMOID: act16_t<PP_ACT_SIGMOID>(v, slope); break;
-    case PP_ACT_TANH: act16_t<PP_ACT_TANH>(v, slope); break;
-    case PP_ACT_GELU: act16_t<PP_ACT_GELU>(v, slope); break;
+    case PP_ACT_RELU: act16_t<PP_ACT_RELU, ACC>(v, slope); break;
+    case PP_ACT_LRELU: act16_t<PP_ACT_LRELU, ACC>(v, slope); break;
+    case PP_ACT_SIGMOID: act16_t<PP_ACT_SIGMOID, ACC>(v, slope); break;
+    case PP_ACT_TANH: act16_t<PP_ACT_TANH, ACC>(v, slope); break;
+    case PP_ACT_GELU: act16_t<PP_ACT_GELU, ACC>(v, slope); break;
     default: break;
   }
 }
@@ -246,7 +249,7 @@ __device__ __forceinline__ void conv_epilogue16_split(const PPConvParams& p, con
   const float* aux1 = reinterpret_cast<const float*>(p.aux1);
   float* out = reinterpret_cast<float*>(p.out);
   if (p.epi == PP_EPI_STD) {
-    act16(v, p.act1, p.slope);
+    act16<true>(v, p.act1, p.slope);
     if (p.scale != 1.f) {
 #pragma unroll
       for (int i = 0; i < 16; ++i) v[i] *= p.scale;
@@ -257,7 +260,7 @@ __device__ __forceinline__ void conv_epilogue16_split(const PPConvParams& p, con
 #pragma unroll
       for (int i = 0; i < 16; ++i) v[i] += r[i];
     }
-    act16(v, p.act2, p.slope);
+    act16<true>(v, p.act2, p.slope);
     float* dst = out + mrow * p.out_cstride + p.out_coff + (long long)g * p.out_gstep + ng0;
     if (p.out_fp32) {
       if (vec && nvalid == 16) {
@@ -274,7 +277,7 @@ __device__ __forceinline__ void conv_epilogue16_split(const PPConvParams& p, con
     }
   } else if (p.epi == PP_EPI_GRU_ZR) {
     const int half_c = p.Cout_g >> 1;
-    act16_t<PP_ACT_SIGMOID>(v, 0.f);
+    act16_t<PP_ACT_SIGMOID, true>(v, 0.f);
     if (ng0 < half_c) {
       store16_split(out + mrow * p.out_cstride + p.out_coff + ng0, p.out_lo, nvalid, vec, v);
     } else {
@@ -289,7 +292,7 @@ __device__ __forceinline__ void conv_epilogue16_split(const PPConvParams& p, con
     float h[16], z[16];
     load16_split(aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, p.aux0_lo, nvalid, vec, h);
     load16_split(aux1 + mrow * p.aux1_cstride + p.aux1_coff + ng0, p.aux1_lo, nvalid, vec, z);
-    act16_t<PP_ACT_TANH>(v, 0.f);
+    act16_t<PP_ACT_TANH, true>(v, 0.f);
 #pragma unroll
     for (int i = 0; i < 16; ++i) v[i] = (1.f - z[i]) * h[i] + z[i] * v[i];
     store16_split(out + mrow * p.out_cstride + p.out_coff + ng0, p.out_lo, nvalid, vec, v);

@@ -265,7 +265,7 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
         mrow = ((long long)t.img * p.OH + oy) * p.OW + ox;
       }
       if (!mvalid || skip || cc >= bnt || n0 + cc >= p.Cout_g) return;
-      if (so != nullptr) {
+      if (!TF32 && so != nullptr) {     // the TMA-store path is fp16 only (HaloParams::tstore)
         // 16 columns = two 16-byte units of panel cc/64, row r, 128B swizzle (unit index XOR row & 7)
         auto slot = [&](int u) {
           const int unit = ((cc & 63) >> 3) + u;

@@ -152,6 +152,15 @@ int pp_comm_all_gather_blocks_impl(PPEngine& e, void* buf, const long long* row_
 // fp32: the split-tf32 path (weights registered under "<name>.tf32", see engine.py); otherwise fp16 activations
 int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
                   bool fp32, cudaStream_t st);
+// RAFT correlation pyramid (raft.cu), shared by pp_stage_raft and pp_op_corr_pyramid.  P_pad: rows of a packed fmap
+// (pp_k_pack_b_operand / _split) of P pixels.
+int pp_raft_corr_pad(int P);
+// All-pairs correlation of `pairs` frame pairs, scaled by 1/sqrt(256): group g correlates fmap g after fmap1 (fp16
+// [P][256], or fp32 split [P][hi 256 | lo 256]) with packed fmap g after fpack2 into corr0 + g*P*P (fp16 / fp32).
+int pp_raft_corr_volume(PPEngine& e, const void* fmap1, const void* fpack2, int pairs, int P, int P_pad, bool fp32,
+                        void* corr0, cudaStream_t st);
+// Levels 1..3 from level 0: 2x2 average pooling of each of the M query maps of h8 x w8
+int pp_raft_corr_pool(PPEngine& e, void* const corr[4], long long M, int h8, int w8, bool fp32, cudaStream_t st);
 int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
                            int H, int W, float* out_f, float* out_b, int team_first, int team_size, cudaStream_t st);
 int pp_stage_image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f,

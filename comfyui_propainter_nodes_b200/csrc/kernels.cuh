@@ -38,7 +38,8 @@ int pp_k_convex_upsample(const float* coords1, const __half* mask, float* out_nc
                          cudaStream_t st);
 // fp32 RAFT path: split-tf32 pair tensors [pix][hi C | lo C] (conv_igemm.cuh), fp32 correlation pyramid
 int pp_k_nchw_f32_to_split(const float* src, float* dst, int N, int C, int H, int W, int cs, cudaStream_t st);
-int pp_k_instnorm_stats_f32(const float* x, int N, int HW, int C, float* sums, cudaStream_t st);
+int pp_k_instnorm_stats_f32(const float* x, int N, int HW, int C, float* sums /*[N][mean C | variance C]*/,
+                            cudaStream_t st);
 int pp_k_instnorm_apply_f32(const float* x, const float* sums, const float* residual, float* out, int N, int HW, int C,
                             int relu, cudaStream_t st);
 int pp_k_pack_b_operand_split(const float* src, float* dst, int G, int R, int R_pad, int K, cudaStream_t st);

@@ -26,9 +26,15 @@ inline int nblocks(long long n, int per = TPB) { return (int)((n + per - 1) / pe
 // result does not depend on scheduling, so RAFT (and everything after it) is bit-reproducible run to run and between
 // the single-GPU and the sharded multi-GPU execution.
 // F32: x is a split pair tensor (float, [pix][hi C | lo C]), else fp16 [pix][C].
+// The fp16 form takes the variance as E[x^2] - mean^2, which cancels for channels whose mean is large against their
+// spread but stays below the fp16 storage rounding up to mean / std ~ 30.  The F32 form runs twice: the first launch
+// leaves the sums of x, the second (`centred`) sums d = x - m1 and d^2 about that first mean m1 and leaves
+// [mean | variance] = [m1 + E[d] | E[d^2] - E[d]^2] (the corrected two-pass algorithm: no cancellation, and the
+// mean is not limited by the rounding of a sum of HW values).
 template <bool F32>
 __global__ void instnorm_stats(const void* __restrict__ xv, int HW, int C, float* __restrict__ sums,
-                               float* __restrict__ partial, unsigned int* __restrict__ counters, int pix_per_block) {
+                               float* __restrict__ partial, unsigned int* __restrict__ counters, int pix_per_block,
+                               int centred) {
   extern __shared__ float sm[];  // [lanes][2C]
   __shared__ bool last;
   const int n = blockIdx.y;
@@ -40,6 +46,12 @@ __global__ void instnorm_stats(const void* __restrict__ xv, int HW, int C, float
   const int p1 = min(HW, p0 + pix_per_block);
   if (pl < lanes) {
     float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+    float m0 = 0.f, m1 = 0.f;
+    if (F32 && centred) {
+      const float inv = 1.f / (float)HW;
+      m0 = sums[(long long)n * 2 * C + 2 * cp] * inv;
+      m1 = sums[(long long)n * 2 * C + 2 * cp + 1] * inv;
+    }
     const __half2* base = reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(xv) + ((long long)n * HW) * C) + cp;
     const float* fbase = reinterpret_cast<const float*>(xv) + ((long long)n * HW) * 2 * C + 2 * cp;
     for (int p = p0 + pl; p < p1; p += lanes) {
@@ -47,11 +59,12 @@ __global__ void instnorm_stats(const void* __restrict__ xv, int HW, int C, float
       if constexpr (F32) {
         const float2 h = *reinterpret_cast<const float2*>(fbase + (long long)p * 2 * C);
         const float2 l = *reinterpret_cast<const float2*>(fbase + (long long)p * 2 * C + C);
-        v = make_float2(h.x + l.x, h.y + l.y);
+        v = make_float2(h.x + l.x - m0, h.y + l.y - m1);
       } else {
         v = __half22float2(base[(long long)p * C2]);
       }
-      s0 += v.x; s1 += v.y; q0 += v.x * v.x; q1 += v.y * v.y;
+      s0 += v.x; s1 += v.y;
+      if (!F32 || centred) { q0 += v.x * v.x; q1 += v.y * v.y; }   // F32: the first pass needs the sums of x only
     }
     float* row = sm + pl * 2 * C;
     row[2 * cp] = s0; row[2 * cp + 1] = s1; row[C + 2 * cp] = q0; row[C + 2 * cp + 1] = q1;
@@ -70,10 +83,25 @@ __global__ void instnorm_stats(const void* __restrict__ xv, int HW, int C, float
   if (last) {
     __threadfence();
     const float* all = partial + (long long)n * gridDim.x * 2 * C;
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
-      float acc = 0.f;
-      for (unsigned b = 0; b < gridDim.x; ++b) acc += __ldcg(all + (long long)b * 2 * C + i);
-      sums[(long long)n * 2 * C + i] = acc;
+    float* out = sums + (long long)n * 2 * C;
+    if (F32 && centred) {   // every block has read m1 before it arrived: out can be overwritten
+      const float inv = 1.f / (float)HW;
+      for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        float ds = 0.f, dq = 0.f;
+        for (unsigned b = 0; b < gridDim.x; ++b) {
+          ds += __ldcg(all + (long long)b * 2 * C + c);
+          dq += __ldcg(all + (long long)b * 2 * C + C + c);
+        }
+        const float dm = ds * inv;
+        out[c] = out[c] * inv + dm;
+        out[C + c] = fmaxf(dq * inv - dm * dm, 0.f);
+      }
+    } else {
+      for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
+        float acc = 0.f;
+        for (unsigned b = 0; b < gridDim.x; ++b) acc += __ldcg(all + (long long)b * 2 * C + i);
+        out[i] = acc;
+      }
     }
   }
 }
@@ -108,9 +136,12 @@ __global__ void __launch_bounds__(256) instnorm_apply(const void* __restrict__ x
   const long long idx = (long long)n * HW * C2 + i;
   const float inv = 1.f / (float)HW;
   const float* s = sums + (long long)n * 2 * C;
-  const float m0 = s[2 * cp] * inv, m1 = s[2 * cp + 1] * inv;
-  const float v0 = fmaxf(s[C + 2 * cp] * inv - m0 * m0, 0.f), v1 = fmaxf(s[C + 2 * cp + 1] * inv - m1 * m1, 0.f);
-  const float r0 = rsqrtf(v0 + 1e-5f), r1 = rsqrtf(v1 + 1e-5f);
+  // F32: s holds [mean | variance] (instnorm_stats, centred), else [sum x | sum x^2]
+  const float m0 = F32 ? s[2 * cp] : s[2 * cp] * inv, m1 = F32 ? s[2 * cp + 1] : s[2 * cp + 1] * inv;
+  const float v0 = F32 ? s[C + 2 * cp] : fmaxf(s[C + 2 * cp] * inv - m0 * m0, 0.f);
+  const float v1 = F32 ? s[C + 2 * cp + 1] : fmaxf(s[C + 2 * cp + 1] * inv - m1 * m1, 0.f);
+  const float r0 = F32 ? __frsqrt_rn(v0 + 1e-5f) : rsqrtf(v0 + 1e-5f);
+  const float r1 = F32 ? __frsqrt_rn(v1 + 1e-5f) : rsqrtf(v1 + 1e-5f);
   // split tensors: pixel idx / C2, channel pair cp
   const long long fo = (long long)n * HW * 2 * C + (long long)(i / (unsigned)C2) * 2 * C + 2 * cp;
   const float2 x2 = F32 ? ld_split2(reinterpret_cast<const float*>(xv) + fo, C)
@@ -304,7 +335,7 @@ __global__ void raft_coords(const float* __restrict__ delta, float* __restrict__
 
 // Convex 8x upsampling (RAFT.upsample_flow, raft.py:81-92): softmax over the 9 neighbours' logits
 // mask[k*64 + sy*8 + sx], weighted sum of 8*flow (3x3 unfold, zero padding).  Output NCHW fp32.
-// T = __half: fp16 mask [q][576]; T = float: split mask [q][hi 576 | lo 576]
+// T = __half: fp16 mask [q][576]; T = float: split mask [q][hi 576 | lo 576], with fp32-accurate exp and division
 template <class T>
 __global__ void convex_upsample(const float* __restrict__ coords1, const T* __restrict__ mask,
                                 float* __restrict__ out, int B, int h8, int w8) {
@@ -328,7 +359,7 @@ __global__ void convex_upsample(const float* __restrict__ coords1, const T* __re
   float den = 0.f, ux = 0.f, uy = 0.f;
 #pragma unroll
   for (int k = 0; k < 9; ++k) {
-    const float e = __expf(lg[k] - mx);
+    const float e = F32 ? ppx::exp_acc(lg[k] - mx) : __expf(lg[k] - mx);
     den += e;
     const int ny = y + k / 3 - 1, nx = x + k % 3 - 1;
     if (ny >= 0 && ny < h8 && nx >= 0 && nx < w8) {
@@ -338,8 +369,8 @@ __global__ void convex_upsample(const float* __restrict__ coords1, const T* __re
     }
   }
   const long long HWl = (long long)H * W;
-  out[((long long)b * 2) * HWl + (long long)Y * W + X] = ux / den;
-  out[((long long)b * 2 + 1) * HWl + (long long)Y * W + X] = uy / den;
+  out[((long long)b * 2) * HWl + (long long)Y * W + X] = F32 ? __fdiv_rn(ux, den) : ux / den;
+  out[((long long)b * 2 + 1) * HWl + (long long)Y * W + X] = F32 ? __fdiv_rn(uy, den) : uy / den;
 }
 
 // ---- fp32 path only --------------------------------------------------------------------------------------------------
@@ -380,7 +411,7 @@ __global__ void cnet_split_f32(const float* __restrict__ c, float* __restrict__ 
   const int ch = idx % 256;
   const long long p = idx / 256;
   const float v = c[p * 512 + ch] + c[p * 512 + 256 + ch];
-  st_split1(hx + p * 2 * hx_C + ch, hx_C, ch < 128 ? tanhf(v) : fmaxf(v, 0.f));
+  st_split1(hx + p * 2 * hx_C + ch, hx_C, ch < 128 ? ppx::tanh_acc(v) : fmaxf(v, 0.f));
 }
 
 // raft_coords of the fp32 path: the flow goes (split) to channels hx_flow_co, +1 of the GRU state only; the motion
@@ -437,7 +468,7 @@ int pp_k_instnorm_stats(const __half* x, int N, int HW, int C, float* sums, cuda
   dim3 grid(nblk, N);
   const int lanes = 256 / (C / 2);
   instnorm_stats<false><<<grid, 256, (size_t)lanes * 2 * C * sizeof(float), st>>>(x, HW, C, sums, partial, counters,
-                                                                                  pix_per_block);
+                                                                                  pix_per_block, 0);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
@@ -448,12 +479,14 @@ int pp_k_instnorm_stats_f32(const float* x, int N, int HW, int C, float* sums, c
   const int nblk = pp_ceil_div(HW, pix_per_block);
   float* partial = sums + (size_t)N * 2 * C;
   unsigned int* counters = reinterpret_cast<unsigned int*>(partial + (size_t)N * nblk * 2 * C);
-  PP_CUDA_CHECK(cudaMemsetAsync(counters, 0, (size_t)N * sizeof(unsigned int), st));
   dim3 grid(nblk, N);
   const int lanes = 256 / (C / 2);
-  instnorm_stats<true><<<grid, 256, (size_t)lanes * 2 * C * sizeof(float), st>>>(x, HW, C, sums, partial, counters,
-                                                                                 pix_per_block);
-  PP_CUDA_CHECK(cudaGetLastError());
+  for (int centred = 0; centred < 2; ++centred) {   // sums of x, then sums of (x - mean)^2
+    PP_CUDA_CHECK(cudaMemsetAsync(counters, 0, (size_t)N * sizeof(unsigned int), st));
+    instnorm_stats<true><<<grid, 256, (size_t)lanes * 2 * C * sizeof(float), st>>>(x, HW, C, sums, partial, counters,
+                                                                                   pix_per_block, centred);
+    PP_CUDA_CHECK(cudaGetLastError());
+  }
   return PP_OK;
 }
 

@@ -212,6 +212,32 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
+// fp32-accurate forms for the fp32 RAFT path.  The library is built with --use_fast_math, which turns tanhf into
+// tanh.approx.f32 (MUFU.TANH, relative error ~2^-11) and expf into ex2.approx of a rounded x*log2(e) (relative error
+// growing with |x|); these stay within a few fp32 ulp.  No IEEE-division slow paths: tanh_acc sits in the conv
+// epilogues.  (sigmoidf_ needs no such form: the error of its rounded x*log2(e) is of the order of the fp32 rounding of
+// x itself, and the split GRU z|r epilogue measures as accurate as torch's fp32 sigmoid.)
+// 1 / d for 1 <= d < 2^126 (finite: at d = inf the Newton step gives NaN): rcp.approx + one Newton step
+__device__ __forceinline__ float rcp_acc(float d) {
+  const float r = __fdividef(1.f, d);
+  return fmaf(fmaf(-d, r, 1.f), r, r);
+}
+// exp(x): the product x*log2(e) is carried to ~2^-48 (fma residual), only ex2.approx's own ~2 ulp remain
+__device__ __forceinline__ float exp_acc(float x) {
+  const float t = x * 1.44269502f;
+  const float r = fmaf(x, 1.44269502f, -t) + x * 1.92596303e-8f;   // x*log2(e) - t
+  return exp2f(t) * fmaf(r, 0.693147181f, 1.f);
+}
+// tanh|x| = expm1(2|x|) / (expm1(2|x|) + 2): no cancellation near 0 (expm1f is not affected by --use_fast_math);
+// tanh(9) rounds to 1 in fp32 (above 9 the quotient, NaN from d = inf, is not selected)
+__device__ __forceinline__ float tanh_acc(float x) {
+  const float a = fabsf(x);
+  const float e = expm1f(2.f * a), d = e + 2.f;
+  float q = e * rcp_acc(d);
+  q = fmaf(fmaf(-q, d, e), rcp_acc(d), q);     // one residual correction of the quotient
+  return copysignf(a > 9.f ? 1.f : q, x);
+}
+
 }  // namespace ppx
 
 #endif  // __CUDACC__

@@ -103,7 +103,7 @@ int enc_conv(Enc& c, const std::string& name, const Act& x, int n, int H, int W,
       PP_TRY(pp_k_instnorm_apply(out.h(), c.sums, residual ? residual->h() : nullptr, out.h(), n, OH * OW, out.C,
                                  relu ? 1 : 0, c.st));
     }
-    c.e.launches += 3;  // memset + 2 kernels
+    c.e.launches += c.f32 ? 5 : 3;  // memset + 2 kernels (fp32: the statistics take two passes)
   } else {
     call.out(out, 0);
     if (residual != nullptr) call.act(relu ? PP_ACT_RELU : PP_ACT_NONE, 0.f, 1.f, PP_ACT_RELU).residual(*residual, 0);
@@ -158,6 +158,65 @@ int encoder(Enc& c, const Act& x, int n, int H, int W, const Act& out) {
 
 }  // namespace
 
+int pp_raft_corr_pad(int P) {
+  const int ntile = pp_ceil_div(P, 256);
+  return ((pp_ceil_div(P, ntile) + 15) / 16) * 16 * ntile;
+}
+
+int pp_raft_corr_volume(PPEngine& e, const void* fmap1, const void* fpack2, int pairs, int P, int P_pad, bool fp32,
+                        void* corr0, cudaStream_t st) {
+  // all-pairs correlation: grouped GEMM, one group per frame pair, scaled by 1/sqrt(256)
+  PP_REQUIRE((long long)P * P < (1LL << 31), "raft: frame too large for the correlation volume indexing");
+  const size_t cb = fp32 ? 4 : 2;
+  const int fk = fp32 ? 3 * 256 : 256;
+  const long long Ms = (long long)pairs * P;
+  PPConvParams p;
+  memset(&p, 0, sizeof(p));
+  if (fp32) {
+    // A = fmap1 read as (hi, lo, hi), in the kernel's 2-byte units (conv_igemm.cuh); B = the [hi; hi; lo] image
+    PP_REQUIRE((long long)pairs * P * 1024 < (1LL << 31), "raft: too many frame pairs for one correlation launch");
+    p.split = 1;
+    p.nseg = 3;
+    for (int k = 0; k < 3; ++k) {
+      p.seg[k].ptr = reinterpret_cast<const __half*>(fmap1);
+      p.seg[k].cstride = 1024; p.seg[k].coff = k == 1 ? 512 : 0;
+      p.seg[k].gstep = P * 1024; p.seg[k].cbegin = 512 * k; p.seg[k].cend = 512 * (k + 1);
+    }
+    p.Cin = 1536;
+  } else {
+    p.nseg = 1;
+    p.seg[0].ptr = reinterpret_cast<const __half*>(fmap1); p.seg[0].cstride = 256; p.seg[0].coff = 0;
+    p.seg[0].gstep = P * 256; p.seg[0].cbegin = 0; p.seg[0].cend = 256;
+    p.Cin = 256;
+  }
+  p.wpacked = reinterpret_cast<const __half*>(fpack2);
+  p.N = 1; p.H = 1; p.W = P; p.OH = 1; p.OW = P;
+  p.kh = p.kw = 1; p.sh = p.sw = 1; p.dh = p.dw = 1;
+  p.bias = nullptr;
+  p.Cout_g = P; p.Cout_g_pad = P_pad; p.BN = P_pad / pp_ceil_div(P, 256); p.groups = pairs;
+  p.epi = PP_EPI_STD; p.scale = 1.f / 16.f;
+  // group g writes rows [g*P, (g+1)*P): out index = m*out_cstride + out_coff + g*out_gstep + n
+  // (P*P exceeds the int range only beyond 46340 pixels at 1/8 res, i.e. 3.7 MPixel frames)
+  p.out = corr0; p.out_cstride = P; p.out_coff = 0; p.out_fp32 = fp32 ? 1 : 0;
+  p.out_gstep = P * P;
+  {
+    PPProfScope ps(e, "conv:igemm:raft.corr", (double)Ms, 2.0 * Ms * P * fk, (double)Ms * P * cb + 2.0 * Ms * fk * cb, st);
+    PP_TRY(pp_launch_conv(p, st));
+  }
+  e.launches++;
+  return PP_OK;
+}
+
+int pp_raft_corr_pool(PPEngine& e, void* const corr[4], long long M, int h8, int w8, bool fp32, cudaStream_t st) {
+  for (int l = 0; l < 3; ++l) {
+    const int h = h8 >> l, w = w8 >> l;
+    if (fp32) PP_TRY(pp_k_corr_pool_f32(static_cast<float*>(corr[l]), static_cast<float*>(corr[l + 1]), M, h, w, st));
+    else PP_TRY(pp_k_corr_pool(static_cast<__half*>(corr[l]), static_cast<__half*>(corr[l + 1]), M, h, w, st));
+    e.launches++;
+  }
+  return PP_OK;
+}
+
 int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
                   bool fp32, cudaStream_t st) {
   PP_REQUIRE(T >= 2, "raft: need at least 2 frames, got %d", T);
@@ -172,11 +231,7 @@ int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int ite
   Act fmap, cmap;
   uint8_t* fpack;
   int P_pad;
-  {
-    const int ntile = pp_ceil_div(P, 256);
-    const int bn = ((pp_ceil_div(P, ntile) + 15) / 16) * 16;
-    P_pad = bn * ntile;
-  }
+  P_pad = pp_raft_corr_pad(P);
   PP_TRY(alloc_act(e, fp32, fmap, (long long)T * P, 256, "fmap"));
   PP_TRY(alloc_act(e, fp32, cmap, (long long)T * P, 256, "cmap"));
   PP_TRY(pp_alloc(e, &fpack, (size_t)T * P_pad * fk * cb, "fmap packed"));
@@ -222,7 +277,6 @@ int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int ite
   int max_pairs = (int)(avail * 9 / 10 / per_pair);
   PP_REQUIRE(max_pairs >= 1, "raft: workspace too small for one frame pair (%zu bytes needed)", per_pair);
   const int npairs = T - 1;
-  const int bn_corr = P_pad / pp_ceil_div(P, 256);
 
   // Both directions share one batch: pair slot s < npairs is the forward pair (s -> s+1), slot npairs + s the backward
   // pair (s+1 -> s).  One launch per layer then covers 2(T-1) pairs (half as many launches and tile-quantisation
@@ -241,59 +295,21 @@ int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int ite
       }
       const size_t m2 = e.arena.mark();
       const long long M = (long long)B * P;
-      uint8_t* corr[4];
-      for (int l = 0; l < 4; ++l) PP_TRY(pp_alloc(e, &corr[l], (size_t)M * lvl_h[l] * lvl_w[l] * cb, "corr level"));
-      // all-pairs correlation: grouped GEMM, one group per frame pair, scaled by 1/sqrt(256)
-      PP_REQUIRE((long long)P * P < (1LL << 31), "raft: frame too large for the correlation volume indexing");
+      void* corr[4];
+      for (int l = 0; l < 4; ++l) {
+        uint8_t* c;
+        PP_TRY(pp_alloc(e, &c, (size_t)M * lvl_h[l] * lvl_w[l] * cb, "corr level"));
+        corr[l] = c;
+      }
       for (int si = 0; si < nsub; ++si) {
         const Sub& sb = subs[si];
         const int f1 = sb.dir == 0 ? sb.b0 : sb.b0 + 1;  // first frame playing image1
         const int f2 = sb.dir == 0 ? sb.b0 + 1 : sb.b0;  // first frame playing image2
-        const long long Ms = (long long)sb.cnt * P;
-        PPConvParams p;
-        memset(&p, 0, sizeof(p));
-        if (fp32) {
-          // A = fmap1 read as (hi, lo, hi), in the kernel's 2-byte units (conv_igemm.cuh); B = the [hi; hi; lo] image
-          PP_REQUIRE((long long)sb.cnt * P * 1024 < (1LL << 31), "raft: too many frame pairs for one correlation launch");
-          p.split = 1;
-          p.nseg = 3;
-          for (int k = 0; k < 3; ++k) {
-            p.seg[k].ptr = reinterpret_cast<const __half*>(fmap.f() + (size_t)f1 * P * 512);
-            p.seg[k].cstride = 1024; p.seg[k].coff = k == 1 ? 512 : 0;
-            p.seg[k].gstep = P * 1024; p.seg[k].cbegin = 512 * k; p.seg[k].cend = 512 * (k + 1);
-          }
-          p.Cin = 1536;
-          p.wpacked = reinterpret_cast<const __half*>(reinterpret_cast<float*>(fpack) + (size_t)f2 * P_pad * 768);
-        } else {
-          p.nseg = 1;
-          p.seg[0].ptr = fmap.h() + (size_t)f1 * P * 256; p.seg[0].cstride = 256; p.seg[0].coff = 0;
-          p.seg[0].gstep = P * 256; p.seg[0].cbegin = 0; p.seg[0].cend = 256;
-          p.Cin = 256;
-          p.wpacked = reinterpret_cast<__half*>(fpack) + (size_t)f2 * P_pad * 256;
-        }
-        p.N = 1; p.H = 1; p.W = P; p.OH = 1; p.OW = P;
-        p.kh = p.kw = 1; p.sh = p.sw = 1; p.dh = p.dw = 1;
-        p.bias = nullptr;
-        p.Cout_g = P; p.Cout_g_pad = P_pad; p.BN = bn_corr; p.groups = sb.cnt;
-        p.epi = PP_EPI_STD; p.scale = 1.f / 16.f;
-        // group g writes rows [g*P, (g+1)*P) of this sub-range: out index = m*out_cstride + out_coff + g*out_gstep + n
-        // (P*P exceeds the int range only beyond 46340 pixels at 1/8 res, i.e. 3.7 MPixel frames)
-        p.out = corr[0] + (size_t)sb.off * P * P * cb; p.out_cstride = P; p.out_coff = 0; p.out_fp32 = fp32 ? 1 : 0;
-        p.out_gstep = P * P;
-        {
-          PPProfScope ps(e, "conv:igemm:raft.corr", (double)Ms, 2.0 * Ms * P * fk,
-                         (double)Ms * P * cb + 2.0 * Ms * fk * cb, st);
-          PP_TRY(pp_launch_conv(p, st));
-        }
-        e.launches++;
+        PP_TRY(pp_raft_corr_volume(e, (const uint8_t*)fmap.p + (size_t)f1 * P * 256 * (fp32 ? 8 : 2),
+                                   fpack + (size_t)f2 * P_pad * fk * cb, sb.cnt, P, P_pad, fp32,
+                                   static_cast<uint8_t*>(corr[0]) + (size_t)sb.off * P * P * cb, st));
       }
-      for (int l = 0; l < 3; ++l) {
-        if (fp32) PP_TRY(pp_k_corr_pool_f32(reinterpret_cast<float*>(corr[l]), reinterpret_cast<float*>(corr[l + 1]), M,
-                                            lvl_h[l], lvl_w[l], st));
-        else PP_TRY(pp_k_corr_pool(reinterpret_cast<__half*>(corr[l]), reinterpret_cast<__half*>(corr[l + 1]), M, lvl_h[l],
-                                   lvl_w[l], st));
-        e.launches++;
-      }
+      PP_TRY(pp_raft_corr_pool(e, corr, M, h8, w8, fp32, st));
       // GRU state and scratch
       Act hx, rh, z, lk, c1, corflo, f1b, fpatch, fh;
       __half* flow8 = nullptr;                 // fp16 only: the flow for the 7x7 patches (fp32 takes it from coords1)
@@ -328,12 +344,12 @@ int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int ite
           // algorithmic bytes per query pixel: coords 8 B + 4 levels x 10x10 taps + 324 outputs (fp32: hi and lo)
           PPProfScope ps(e, "corr_lookup", (double)M, 0.0, (double)M * (8 + 4 * 100 * cb + 324 * (fp32 ? 8 : 2)), st);
           if (fp32)
-            PP_TRY(pp_k_corr_lookup_f32(reinterpret_cast<float*>(corr[0]), reinterpret_cast<float*>(corr[1]),
-                                        reinterpret_cast<float*>(corr[2]), reinterpret_cast<float*>(corr[3]), coords1,
+            PP_TRY(pp_k_corr_lookup_f32(static_cast<float*>(corr[0]), static_cast<float*>(corr[1]),
+                                        static_cast<float*>(corr[2]), static_cast<float*>(corr[3]), coords1,
                                         lk.f(), lk_C, M, h8, w8, st));
           else
-            PP_TRY(pp_k_corr_lookup(reinterpret_cast<__half*>(corr[0]), reinterpret_cast<__half*>(corr[1]),
-                                    reinterpret_cast<__half*>(corr[2]), reinterpret_cast<__half*>(corr[3]), coords1, lk.h(),
+            PP_TRY(pp_k_corr_lookup(static_cast<__half*>(corr[0]), static_cast<__half*>(corr[1]),
+                                    static_cast<__half*>(corr[2]), static_cast<__half*>(corr[3]), coords1, lk.h(),
                                     lk_C, M, P, h8, w8, st));
         }
         e.launches++;

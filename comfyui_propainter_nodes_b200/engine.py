@@ -60,6 +60,12 @@ _SIGNATURES = {
     "pp_profile_dump": (_I, [_VP, ctypes.c_char_p, _SZ]),
     "pp_op_conv": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _F, _VP, _VP, _VP]),
     "pp_op_corr_lookup": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
+    "pp_op_conv_tf32": (_I, [_VP, _CP, _VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _I,
+                             _VP, _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _VP]),
+    "pp_op_instnorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "pp_op_corr_pyramid": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
+    "pp_op_corr_lookup_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
+    "pp_op_convex_upsample": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "pp_op_imgprop_step": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP]),
     "pp_op_attention": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
 }
@@ -752,6 +758,63 @@ class Engine:
         out = torch.empty(nq, 328, device=self.device, dtype=torch.float16)
         self._check(self.lib.pp_op_corr_lookup(self.h, *[_ptr(l) for l in levels], _ptr(coords), _ptr(out), nq, h8, w8,
                                                self._stream()))
+        return out
+
+    EPI_STD, EPI_GRU_ZR, EPI_GRU_H = range(3)
+
+    def op_conv_tf32(self, name, inputs, out, out_co=0, stride=(1, 1), pad=(0, 0), act=ACT_NONE, slope=0.0, scale=1.0,
+                     act2=ACT_NONE, residual=None, gru_zr=None, gru_h=None, out_fp32=False):
+        """One split-tf32 convolution (weights from register_conv_tf32) on split tensors [N,H,W,2C] float32 (split_tf32:
+        hi channels, then lo).  inputs: one or two (tensor, first channel, channels); out: split tensor written at channel
+        out_co, or with out_fp32 a plain [N,OH,OW,C] float32 tensor.  Epilogue: act / slope / scale / act2 and an optional
+        residual (tensor, co); or gru_zr = (h, h_co, rh, rh_co) (z -> out, r * h -> rh); or gru_h = (h, h_co, z, z_co)."""
+        N, H, W = inputs[0][0].shape[:3]
+        (x0, c0, n0), (x1, c1, n1) = inputs[0], (inputs[1] if len(inputs) > 1 else (None, 0, 0))
+        C = lambda t: 0 if t is None else t.shape[-1] // 2
+        epi, a0, a0_co, a1, a1_co = self.EPI_STD, None, 0, None, 0
+        if residual is not None:
+            a0, a0_co = residual
+        if gru_zr is not None:
+            epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_ZR, gru_zr
+        if gru_h is not None:
+            epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_H, gru_h
+        self._check(self.lib.pp_op_conv_tf32(
+            self.h, (name + ".tf32").encode(), _ptr(x0), C(x0), c0, n0, _ptr(x1), C(x1), c1, n1, N, H, W, stride[0],
+            stride[1], pad[0], pad[1], epi, act, float(slope), float(scale), act2, _ptr(a0), C(a0), a0_co, _ptr(a1), C(a1),
+            a1_co, _ptr(out), out.shape[-1] if out_fp32 else C(out), out_co, int(out_fp32), self._stream()))
+        return out
+
+    def op_instnorm(self, x, C, relu=False, residual=None, out=None, fp32=True):
+        """InstanceNorm2d of x [N,HW,C] fp16 (fp32=False) or [N,HW,2C] split float32, + relu, then relu(residual + .)."""
+        out = torch.empty_like(x) if out is None else out
+        N, HW = x.shape[:2]
+        self._check(self.lib.pp_op_instnorm(self.h, _ptr(x), _ptr(residual), _ptr(out), N, HW, C, int(relu), int(fp32),
+                                            self._stream()))
+        return out
+
+    def op_corr_pyramid(self, fmap1, fmap2, h8, w8, fp32=True):
+        """fmap1 / fmap2 [pairs, h8*w8, 256] fp16 or [pairs, h8*w8, 512] split float32 -> the 4 pyramid levels
+        [pairs*h8*w8, (h8 >> l) * (w8 >> l)] (fp16 / float32)."""
+        pairs = fmap1.shape[0]
+        dt = torch.float32 if fp32 else torch.float16
+        lv = [torch.empty(pairs * h8 * w8, (h8 >> l) * (w8 >> l), device=self.device, dtype=dt) for l in range(4)]
+        self._check(self.lib.pp_op_corr_pyramid(self.h, _ptr(fmap1), _ptr(fmap2), pairs, h8, w8, int(fp32),
+                                                *[_ptr(t) for t in lv], self._stream()))
+        return lv
+
+    def op_corr_lookup_f32(self, levels, coords, h8, w8):
+        """fp32 pyramid -> split [nq, 704] float32 (hi 352 | lo 352)."""
+        nq = coords.shape[0]
+        out = torch.empty(nq, 704, device=self.device, dtype=torch.float32)
+        self._check(self.lib.pp_op_corr_lookup_f32(self.h, *[_ptr(l) for l in levels], _ptr(coords), _ptr(out), nq, h8,
+                                                   w8, self._stream()))
+        return out
+
+    def op_convex_upsample(self, coords1, mask, B, h8, w8, fp32=True):
+        """coords1 [B*h8*w8, 2], mask [B*h8*w8, 576] fp16 or [B*h8*w8, 1152] split float32 -> [B, 2, 8*h8, 8*w8]."""
+        out = torch.empty(B, 2, 8 * h8, 8 * w8, device=self.device, dtype=torch.float32)
+        self._check(self.lib.pp_op_convex_upsample(self.h, _ptr(coords1), _ptr(mask), _ptr(out), B, h8, w8, int(fp32),
+                                                   self._stream()))
         return out
 
     def op_imgprop_step(self, cur4, prop4, flow_prop, flow_check):

@@ -155,6 +155,32 @@ PP_API int pp_op_conv(pp_handle h, const char* name, const void* x_f16, int N, i
                int replicate, int act, float slope, const void* residual_f16, void* out_f16, void* stream);
 PP_API int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream);
+/* Operators of the fp32 RAFT path (pp_raft_bidir_fp32).  Split tensors are fp32 [pix][hi C | lo C] with hi = tf32(x),
+ * lo = x - hi; `*_C` is a tensor's channel count C, `*_co` / `*_ch` count channels.
+ * One split-tf32 convolution with weights registered as a split image (Engine.register_conv_tf32): input x0 channels
+ * [x0_co, x0_co + x0_ch) (then x1's, when x1 is not null), stride sh x sw, zero padding ph x pw, epilogue
+ * epi = 0: act2(act(acc + bias) * scale + aux0), aux0 an optional split residual;
+ * epi = 1 (GRU z|r): z -> out, r * aux0 (h) -> aux1 (r*h);  epi = 2 (GRU q): (1 - z) * h + z * tanh(acc + bias) -> out
+ * with h = aux0, z = aux1.  out is split, written at channel out_co, or (out_fp32) plain fp32 [pix][out_C]. */
+PP_API int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, int x0_co, int x0_ch, const float* x1,
+                           int x1_C, int x1_co, int x1_ch, int N, int H, int W, int sh, int sw, int ph, int pw, int epi,
+                           int act, float slope, float scale, int act2, const float* aux0, int aux0_C, int aux0_co,
+                           float* aux1, int aux1_C, int aux1_co, float* out, int out_C, int out_co, int out_fp32,
+                           void* stream);
+/* InstanceNorm2d (eps 1e-5, no affine) of N images [HW][C] (+relu) (then relu(residual + .)): fp16 [pix][C] or, with
+ * fp32, split tensors.  out may be x. */
+PP_API int pp_op_instnorm(pp_handle h, const void* x, const void* residual, void* out, int N, int HW, int C, int relu,
+                          int fp32, void* stream);
+/* RAFT correlation pyramid of `pairs` frame pairs: fmap1 / fmap2 [pairs][h8*w8][256] (fp16, or with fp32 split) ->
+ * levels l0..l3 [pairs*h8*w8][(h8 >> l) * (w8 >> l)] (fp16 / fp32). */
+PP_API int pp_op_corr_pyramid(pp_handle h, const void* fmap1, const void* fmap2, int pairs, int h8, int w8, int fp32,
+                              void* l0, void* l1, void* l2, void* l3, void* stream);
+/* pp_op_corr_lookup on an fp32 pyramid: out is split [nq][hi 352 | lo 352] (channels 324..351 zero). */
+PP_API int pp_op_corr_lookup_f32(pp_handle h, const float* l0, const float* l1, const float* l2, const float* l3,
+                                 const float* coords, float* out, long long nq, int h8, int w8, void* stream);
+/* RAFT convex 8x upsampling: coords1 [B*h8*w8][2], mask [B*h8*w8][576] fp16 (or with fp32 split) -> out [B][2][8h8][8w8]. */
+PP_API int pp_op_convex_upsample(pp_handle h, const float* coords1, const void* mask, float* out, int B, int h8, int w8,
+                                 int fp32, void* stream);
 PP_API int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* prop_in4_f16, void* prop_out4_f16,
                        const void* flow_prop_f16, const void* flow_check_f16, int H, int W, void* stream);
 PP_API int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,
