@@ -334,8 +334,9 @@ __device__ __forceinline__ void drain_acc(const float (&acc)[N / 2], float* stg,
   }
 }
 
-// conv_epilogue16 (SPLIT: conv_epilogue16_split) on 16 staged accumulators
-template <bool SPLIT = false>
+// conv_epilogue16 (SPLIT: conv_epilogue16_split) on 16 staged accumulators.  EPI >= 0: the layer's epilogue kind, known
+// at compile time (only that branch of conv_epilogue16 is generated); -1: p.epi at run time.
+template <bool SPLIT = false, int EPI = -1>
 __device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const float* src, long long mrow, int g, int ng0,
                                                     uint4* sm0, uint4* sm1) {
   if constexpr (SPLIT) {
@@ -354,7 +355,7 @@ __device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const
       raw[i] = __float_as_uint(v.x); raw[i + 1] = __float_as_uint(v.y);
       raw[i + 2] = __float_as_uint(v.z); raw[i + 3] = __float_as_uint(v.w);
     }
-    conv_epilogue16(p, raw, mrow, g, ng0, p.epi, p.vec_ok != 0, nullptr, sm0, sm1);
+    conv_epilogue16(p, raw, mrow, g, ng0, EPI >= 0 ? EPI : p.epi, p.vec_ok != 0, nullptr, sm0, sm1);
   }
 }
 

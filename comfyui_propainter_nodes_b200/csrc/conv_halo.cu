@@ -162,40 +162,33 @@ __device__ __forceinline__ void halo_tap(float (&acc)[MB][BN / 2], uint64_t (&ad
   for (int b = 0; b < MB; ++b) adesc[b] += step;
 }
 
-// The wgmmas of one weight stage (tn filter taps) as one commit group.
-// NT > 0 (tn <= NT): the tap count is dispatched to a compile-time constant, so the group is straight-line code.  A
-// runtime-length tap loop puts the group's wgmmas on several control paths; ptxas then injects warpgroup.arrive at the
-// joins (C7519 / C7520) and makes every wgmma wait for the previous one.
-// NT == 0: that runtime loop, for conv_prog_kernel, whose wgmmas ptxas serializes for lack of registers anyway (C7512)
-// and where the unrolled groups only add spills.
+// The wgmmas of one weight stage (tn <= NT filter taps) as one commit group.  The tap count is dispatched to a
+// compile-time constant, so the group is straight-line code.  A runtime-length tap loop puts the group's wgmmas on
+// several control paths; ptxas then injects warpgroup.arrive at the joins (C7519 / C7520) and makes every wgmma wait
+// for the previous one.
 template <int BN, int MB, int NT, bool TF32>
 __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2], uint64_t (&adesc)[MB], uint64_t bdesc,
                                                uint32_t& accum, int& kx, int kw, uint32_t step_x, uint32_t step_row,
                                                uint32_t tap16) {
   using namespace ppx;
-  if constexpr (NT == 0) {
-    wgmma_fence();
-    for (int tt = 0; tt < tn; ++tt) halo_tap<BN, MB, TF32>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
-    wgmma_commit();
-  } else {
-    if constexpr (NT > 1) {
-      if (tn < NT) {
-        halo_tap_group<BN, MB, NT - 1, TF32>(tn, acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
-        return;
-      }
+  if constexpr (NT > 1) {
+    if (tn < NT) {
+      halo_tap_group<BN, MB, NT - 1, TF32>(tn, acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+      return;
     }
-    wgmma_fence();
-#pragma unroll
-    for (int tt = 0; tt < NT; ++tt) halo_tap<BN, MB, TF32>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
-    wgmma_commit();
   }
+  wgmma_fence();
+#pragma unroll
+  for (int tt = 0; tt < NT; ++tt) halo_tap<BN, MB, TF32>(acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+  wgmma_commit();
 }
 
 // Consumer side of one tile, run by each of the two consumer warpgroups: the main loop into register accumulators
 // (MB = h.MT m64 blocks of BN columns), then the epilogue of this warpgroup's pixel rows.  A stage is handed back to
 // its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
-// NT: see halo_tap_group.  TF32: the split-tf32 form.
-template <int BN, int MB, int NT, bool TF32 = false>
+// NT: see halo_tap_group.  TF32: the split-tf32 form.  PROG (conv_prog_kernel): the layer has the plain epilogue
+// (PP_EPI_STD) and no TMA-store staging tile, so neither the GRU epilogues nor the TMA-store path are compiled in.
+template <int BN, int MB, int NT, bool TF32 = false, bool PROG = false>
 __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
                                           int wg, int t128) {
   using namespace ppx;
@@ -244,7 +237,7 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
   const bool skip = (h.debug & 1) != 0;
   const int bar_id = 2 + (MB == 2 ? wg : 0), bar_n = MB == 2 ? 128 : 256;
   const bool issuer = t128 == 0 && (MB == 2 || wg == 0);
-  uint8_t* so = h.tstore ? m.out_stg + (MB == 2 ? wg : 0) * h.out_stage_bytes : nullptr;
+  uint8_t* so = !PROG && h.tstore ? m.out_stg + (MB == 2 ? wg : 0) * h.out_stage_bytes : nullptr;
   if (so != nullptr) {
     if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
     named_bar(bar_id, bar_n);
@@ -273,7 +266,7 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
         };
         ppconv::epilogue_from_stage(p, src, mrow, t.g, n0 + cc, slot(0), slot(1));
       } else {
-        ppconv::epilogue_from_stage<TF32>(p, src, mrow, t.g, n0 + cc, nullptr, nullptr);
+        ppconv::epilogue_from_stage<TF32, PROG ? PP_EPI_STD : -1>(p, src, mrow, t.g, n0 + cc, nullptr, nullptr);
       }
     });
   }
@@ -422,6 +415,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_halo_tf32_kernel(const __
 constexpr int PROG_MAX_LAYERS = 10;
 enum { PROG_CONV = 0, PROG_DCN = 1 };
 
+// The N tile widths of program layers (all with MT == 1), the ones the plan of halo_configure (one_wave) picks for the
+// propagation steps of flow completion: two clips (D = 2, 7,200 pixels at 640x360) take 64 for the 128-channel layers and
+// 224 for the 432-channel offset head (2 N tiles: one wave), one clip (D = 1) takes 32 and 64.  Each width instantiates
+// the whole main loop and epilogue in the consumer warpgroups' 232 registers, so the list is kept this short: all eight
+// widths up to 128 made the kernel spill and ptxas serialize its wgmmas, and 112 next to 224 spills too.
+constexpr int PROG_WIDTHS[] = {32, 64, 224};
+
+template <class F>
+__device__ __forceinline__ void with_prog_width(int bn, F&& f) {
+  static_assert(sizeof(PROG_WIDTHS) == 3 * sizeof(int), "with_prog_width: one case per PROG_WIDTHS entry");
+  switch (bn) {
+    case PROG_WIDTHS[0]: f(ppconv::IntC<PROG_WIDTHS[0]>{}); break;
+    case PROG_WIDTHS[1]: f(ppconv::IntC<PROG_WIDTHS[1]>{}); break;
+    case PROG_WIDTHS[2]: f(ppconv::IntC<PROG_WIDTHS[2]>{}); break;
+    default: __trap();
+  }
+}
+
 struct ProgParams {
   int n_layers;
   int SA, SB, a_stage_bytes, b_stage_bytes;   // one shared-memory carve-up for every layer
@@ -502,11 +513,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
       } else {
         const HaloParams& h = P.layer[li];
         const int total_tiles = halo_total_tiles(h);
-        // program layers are configured with MT == 1 and BN <= 128 (halo_configure, one_wave): wider or two-sub-tile
-        // instances make this kernel spill its accumulators
-        ppconv::with_tile_width<128>(h.c.BN, [&](auto bn) {
+        // program layers are configured with MT == 1 and BN in PROG_WIDTHS (halo_configure, one_wave)
+        with_prog_width(h.c.BN, [&](auto bn) {
+          constexpr int BN = decltype(bn)::value;
           for (int tile = blockIdx.x; tile < total_tiles; tile += G)
-            halo_tile<decltype(bn)::value, 1, 0>(h, tile, m, ra, rb, stg, wg, t128);
+            halo_tile<BN, 1, halo_max_tps(BN), false, true>(h, tile, m, ra, rb, stg, wg, t128);
         });
       }
       // publish this CTA's part of the layer: stores -> async proxy, CTA-wide meet of the writers, one arrival
@@ -639,8 +650,8 @@ int halo_launch(void (*kernel)(Params), const Params& params, int grid, int smem
 }
 
 // Tile shape, pipeline depth and tensor maps of one layer.  one_wave: the layer is one of a multi-layer program whose
-// layers are separated by grid-wide barriers -- prefer a tile count just below the SM count (a second, partial wave
-// doubles the layer's latency) over fewer weight re-reads.
+// layers are separated by grid-wide barriers -- prefer the least work per CTA (a second, partial wave doubles the
+// layer's latency) over fewer weight re-reads, among the tile widths the program kernel instantiates.
 int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   h.c = pin;
   PPConvParams& p = h.c;
@@ -659,13 +670,18 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   int mt = count(2, bn) < num_sms ? 1 : 2;
   while (count(mt, bn) < num_sms && bn >= 64 && bn % 32 == 0) bn /= 2;   // small launches: more, narrower tiles
   if (one_wave) {
-    // largest tile count that still fits one wave: 128-pixel tiles, N split into 1..8 tiles of <= 128 columns (the
-    // only shapes the program kernel instantiates; the fallback bn above is <= 128 too)
+    // 128-pixel tiles of a width the program kernel instantiates (PROG_WIDTHS).  The layer takes as long as the CTA with
+    // the most work, waves x BN columns: the width that makes that smallest, among equals the one with fewer waves.
+    // At 640x360 with two clips this puts every layer of a propagation step in one wave of <= 132 tiles.
     mt = 1;
-    for (int nt = 8; nt >= 1; --nt) {
-      const int b = pp_ceil_div(pp_ceil_div(p.Cout_g_pad, nt), 16) * 16;
-      if (b > 128 || b < 16) continue;
-      if (count(1, b) <= num_sms) { mt = 1; bn = b; break; }
+    long long best_cols = -1, best_waves = 0;
+    for (const int b : PROG_WIDTHS) {
+      const long long waves = (count(1, b) + num_sms - 1) / num_sms;
+      if (best_cols < 0 || waves * b < best_cols || (waves * b == best_cols && waves < best_waves)) {
+        best_cols = waves * b;
+        best_waves = waves;
+        bn = b;
+      }
     }
   }
   p.BN = bn;
@@ -782,10 +798,12 @@ int pp_prog_record_conv(const PPConvParams& p) {
   PP_REQUIRE(r->prog.n_layers < PROG_MAX_LAYERS, "conv program: more than %d layers", PROG_MAX_LAYERS);
   PP_REQUIRE(pp_conv_halo_eligible(p), "conv program: layer is not a stride-1 TMA halo-kernel convolution");
   PP_REQUIRE(!p.split, "conv program: split-tf32 layers are not supported");
+  PP_REQUIRE(p.epi == PP_EPI_STD, "conv program: only the plain epilogue (bias, activations, residual) is compiled in");
   const int li = r->prog.n_layers;
   PP_TRY(halo_configure(p, r->prog.layer[li], true));
-  PP_REQUIRE(r->prog.layer[li].MT == 1 && r->prog.layer[li].c.BN <= 128, "conv program: layer tile %d x %d columns",
-             r->prog.layer[li].MT, r->prog.layer[li].c.BN);
+  const HaloParams& h = r->prog.layer[li];
+  PP_REQUIRE(h.MT == 1 && !h.tstore && (h.c.BN == PROG_WIDTHS[0] || h.c.BN == PROG_WIDTHS[1] || h.c.BN == PROG_WIDTHS[2]),
+             "conv program: layer tile %d x %d columns is not instantiated", h.MT, h.c.BN);
   r->prog.kind[li] = PROG_CONV;
   r->prog.n_layers++;
   r->n_conv++;
