@@ -198,7 +198,18 @@ int pp_image_propagate(pp_handle h, const float* frames, const float* masks, con
   PP_REQUIRE(frames && masks && flows_f && flows_b && updated_frames && updated_masks,
              "pp_image_propagate: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_image_propagate(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks,
+  return pp_stage_image_propagate(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks, false,
+                                  as_stream(stream));
+}
+
+int pp_image_propagate_fp32(pp_handle h, const float* frames, const float* masks, const float* flows_f,
+                            const float* flows_b, int T, int H, int W, float* updated_frames, float* updated_masks,
+                            void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(frames && masks && flows_f && flows_b && updated_frames && updated_masks,
+             "pp_image_propagate_fp32: null pointer");
+  ArenaGuard guard(e.arena);
+  return pp_stage_image_propagate(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks, true,
                                   as_stream(stream));
 }
 
@@ -508,6 +519,14 @@ int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* prop_in4_f
   return pp_k_imgprop_step(static_cast<const __half*>(cur4_f16), static_cast<const __half*>(prop_in4_f16),
                            static_cast<__half*>(prop_out4_f16), static_cast<const __half*>(flow_prop_f16),
                            static_cast<const __half*>(flow_check_f16), H, W, as_stream(stream));
+}
+
+int pp_op_imgprop_step_f32(pp_handle h, const float* cur4, const float* prop_in4, float* prop_out4,
+                           const float* flow_prop, const float* flow_check, int H, int W, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(cur4 && prop_in4 && prop_out4 && flow_prop && flow_check, "pp_op_imgprop_step_f32: null pointer");
+  e.launches++;
+  return pp_k_imgprop_step_f32(cur4, prop_in4, prop_out4, flow_prop, flow_check, H, W, as_stream(stream));
 }
 
 int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,

@@ -163,8 +163,9 @@ int pp_raft_corr_volume(PPEngine& e, const void* fmap1, const void* fpack2, int 
 int pp_raft_corr_pool(PPEngine& e, void* const corr[4], long long M, int h8, int w8, bool fp32, cudaStream_t st);
 int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
                            int H, int W, float* out_f, float* out_b, int team_first, int team_size, cudaStream_t st);
+// fp32: frames / masks stored as float4 and flows as float2 (the node's fp16="disable"), else 4 x fp16 / __half2
 int pp_stage_image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f,
-                             const float* flows_b, int T, int H, int W, float* upd_frames, float* upd_masks,
+                             const float* flows_b, int T, int H, int W, float* upd_frames, float* upd_masks, bool fp32,
                              cudaStream_t st);
 int pp_stage_gen_begin(PPEngine& e, const float* frames, const float* masks_in, const float* masks_upd,
                  const float* flows_f, const float* flows_b, int T, int H, int W, const unsigned char* need,

@@ -63,6 +63,15 @@ int pp_k_imgprop_pack(const float* frames, const float* masks, __half* dst, int 
 int pp_k_imgprop_finish(const __half* prop, const float* frames, const float* masks, float* upd_frames,
                         float* upd_masks, int T, int H, int W, cudaStream_t st);
 int pp_k_flow_to_nhwc2(const float* src, __half* dst, int n, int H, int W, cudaStream_t st);
+// fp32 image propagation: pixels float4 (r, g, b, mask), flows float2, fp32 sums in PyTorch's order
+int pp_k_imgprop_step_f32(const float* cur, const float* prop_in, float* prop_out, const float* flow_prop,
+                          const float* flow_check, int H, int W, cudaStream_t st);
+int pp_k_imgprop_run_f32(const float* in4, float* bwd, float* fwd, const float* ff, const float* fbk,
+                         const float* masks, int T, int H, int W, int* scratch, cudaStream_t st);
+int pp_k_imgprop_pack_f32(const float* frames, const float* masks, float* dst, int T, int H, int W, cudaStream_t st);
+int pp_k_imgprop_finish_f32(const float* prop, const float* frames, const float* masks, float* upd_frames,
+                            float* upd_masks, int T, int H, int W, cudaStream_t st);
+int pp_k_flow_to_nhwc2_f32(const float* src, float* dst, int n, int H, int W, cudaStream_t st);
 int pp_k_rfc_pack_input(const float* flows, const float* masks, __half* dst, long long dst_tstride_pix, int T, int H,
                         int W, int reverse_time, cudaStream_t st);
 int pp_k_rfc_combine(const __half* pred, int pred_cs, long long pred_tstride_pix, const float* gt, const float* masks,

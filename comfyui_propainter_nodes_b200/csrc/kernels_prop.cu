@@ -25,6 +25,10 @@ struct Bilin {
   float w00, w01, w10, w11;  // weights, already zero for out-of-range corners
 };
 
+// The weights are ATen's CPU form (w = x - floor(x), e = 1 - w; nw = s * e ...).  ATen's CUDA form ((ix_se - ix) *
+// (iy_se - iy) ...) gives the same weight on every in-range corner: for floor(sx) >= 0, sx - floor(sx) is exact, so
+// both round the same exact value once; they differ only for floor(sx) = -1, on the weight of column -1, which is out
+// of range and zeroed here.
 __device__ __forceinline__ Bilin bilin_setup(float sx, float sy, int W, int H) {
   Bilin b;
   const float fx = floorf(sx), fy = floorf(sy);
@@ -56,6 +60,74 @@ __device__ __forceinline__ float fb_valid(float2 fp, float2 fcw) {
   return (dx * dx + dy * dy) < (0.01f * mag + 0.5f) ? 1.f : 0.f;
 }
 
+// fp32 forms of sample_flow2 / fb_valid for the fp32 image propagation: every product and sum rounded on its own, in
+// the order torch's CPU fp32 evaluation uses (grid_sample's nw + ne + sw + se; fbConsistencyCheck's per-tensor ops),
+// so the discrete decisions downstream (fb test, 0.1 threshold) are the ones the reference takes on the CPU.  No FMA
+// contraction.  (ATen's CUDA grid_sample is compiled with contraction, so it can round these sums differently.)
+__device__ __forceinline__ float2 sample_flow2_rn(const float2* f, const Bilin& b, int W) {
+  float2 r = make_float2(0.f, 0.f);
+  auto acc = [&](float w, float2 v) { r.x = __fadd_rn(r.x, __fmul_rn(w, v.x)); r.y = __fadd_rn(r.y, __fmul_rn(w, v.y)); };
+  if (b.w00 != 0.f) acc(b.w00, f[b.y0 * W + b.x0]);
+  if (b.w01 != 0.f) acc(b.w01, f[b.y0 * W + b.x0 + 1]);
+  if (b.w10 != 0.f) acc(b.w10, f[(b.y0 + 1) * W + b.x0]);
+  if (b.w11 != 0.f) acc(b.w11, f[(b.y0 + 1) * W + b.x0 + 1]);
+  return r;
+}
+
+__device__ __forceinline__ float fb_valid_rn(float2 fp, float2 fcw) {
+  const float dx = __fadd_rn(fp.x, fcw.x), dy = __fadd_rn(fp.y, fcw.y);
+  const float mag = __fadd_rn(__fadd_rn(__fmul_rn(fp.x, fp.x), __fmul_rn(fp.y, fp.y)),
+                              __fadd_rn(__fmul_rn(fcw.x, fcw.x), __fmul_rn(fcw.y, fcw.y)));
+  return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < __fadd_rn(__fmul_rn(0.01f, mag), 0.5f) ? 1.f : 0.f;
+}
+
+// Storage of the image-propagation kernels.  A pixel is (r, g, b, mask) in one vector access: 4 x fp16 (uint2) on the
+// fp16 path, float4 on the fp32 path (the node's fp16="disable"); flows are __half2 / float2.  The fp32 form also runs
+// the bilinear sums and the fb test through the *_rn forms above.
+struct ImgF16 {
+  using Pix = uint2;
+  using Flow = __half2;
+  static constexpr bool exact = false;
+  __device__ static float2 flow(Flow f) { return __half22float2(f); }
+  __device__ static float2 rg(const Pix& t) { return __half22float2(*reinterpret_cast<const __half2*>(&t.x)); }
+  __device__ static float2 bm(const Pix& t) { return __half22float2(*reinterpret_cast<const __half2*>(&t.y)); }
+  __device__ static float mask_of(const Pix& t) { return __half2float(reinterpret_cast<const __half*>(&t)[3]); }
+  __device__ static float mask_at(const Pix* p, int i) { return __half2float(reinterpret_cast<const __half*>(&p[i])[3]); }
+  __device__ static Pix make(float r, float g, float b, float m) {
+    uint2 o;
+    *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(r, g);
+    *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(b, m);
+    return o;
+  }
+  __device__ static Flow make_flow(float x, float y) { return __floats2half2_rn(x, y); }
+};
+
+struct ImgF32 {
+  using Pix = float4;
+  using Flow = float2;
+  static constexpr bool exact = true;
+  __device__ static float2 flow(Flow f) { return f; }
+  __device__ static float2 rg(const Pix& t) { return make_float2(t.x, t.y); }
+  __device__ static float2 bm(const Pix& t) { return make_float2(t.z, t.w); }
+  __device__ static float mask_of(const Pix& t) { return t.w; }
+  __device__ static float mask_at(const Pix* p, int i) { return reinterpret_cast<const float*>(&p[i])[3]; }
+  __device__ static Pix make(float r, float g, float b, float m) { return make_float4(r, g, b, m); }
+  __device__ static Flow make_flow(float x, float y) { return make_float2(x, y); }
+};
+
+template <class S>
+__device__ __forceinline__ float fb_valid_of(float2 fp, const typename S::Flow* fchk, const Bilin& b, int W) {
+  if constexpr (S::exact) return fb_valid_rn(fp, sample_flow2_rn(fchk, b, W));
+  else return fb_valid(fp, sample_flow2(fchk, b, W));
+}
+
+// bilinear mask sum: w * m over the non-zero corners in grid_sample's order (nw, ne, sw, se)
+template <class S>
+__device__ __forceinline__ void mask_acc(float& mw, float w, float m) {
+  if constexpr (S::exact) mw = __fadd_rn(mw, __fmul_rn(w, m));
+  else mw += w * m;
+}
+
 // ------------------------------------------------------------------------------------------------
 // One time step of the non-learnable image propagation (BidirectionalPropagation(3, learnable=False),
 // model/propainter.py:157-196), fully fused: fb check, nearest warp of the propagated pixels, bilinear
@@ -63,43 +135,41 @@ __device__ __forceinline__ float fb_valid(float2 fp, float2 fcw) {
 // Pixel layout: 4 x fp16 = (r, g, b, mask) so one 8-byte access moves a whole pixel.
 // Algorithmic traffic: cur 8 B + prop gather 8 B (+ 3 more mask taps) + out 8 B + 2 flows 4 B each.
 // ------------------------------------------------------------------------------------------------
-__global__ void imgprop_step(const uint2* __restrict__ cur, const uint2* __restrict__ prop_in,
-                             uint2* __restrict__ prop_out, const __half2* __restrict__ flow_prop,
-                             const __half2* __restrict__ flow_check, int H, int W) {
+template <class S>
+__global__ void imgprop_step(const typename S::Pix* __restrict__ cur, const typename S::Pix* __restrict__ prop_in,
+                             typename S::Pix* __restrict__ prop_out, const typename S::Flow* __restrict__ flow_prop,
+                             const typename S::Flow* __restrict__ flow_check, int H, int W) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= H * W) return;
   const int x = idx % W, y = idx / W;
-  const float2 fp = __half22float2(flow_prop[idx]);
+  const float2 fp = S::flow(flow_prop[idx]);
   const float sx = sample_coord((float)x + fp.x, W), sy = sample_coord((float)y + fp.y, H);
   const Bilin b = bilin_setup(sx, sy, W, H);
-  const float valid = fb_valid(fp, sample_flow2(flow_check, b, W));
+  const float valid = fb_valid_of<S>(fp, flow_check, b, W);
   // nearest texel of the propagated frame
   const int nx = (int)nearbyintf(sx), ny = (int)nearbyintf(sy);
   float wr = 0.f, wg = 0.f, wb = 0.f;
   if (nx >= 0 && nx < W && ny >= 0 && ny < H) {
-    const uint2 t = prop_in[ny * W + nx];
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x));
-    const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
+    const typename S::Pix t = prop_in[ny * W + nx];
+    const float2 a = S::rg(t);
+    const float2 c = S::bm(t);
     wr = a.x; wg = a.y; wb = c.x;
   }
   // bilinear sample of the propagated mask (4th channel)
   float mw = 0.f;
-  if (b.w00 != 0.f) mw += b.w00 * __half2float(reinterpret_cast<const __half*>(&prop_in[b.y0 * W + b.x0])[3]);
-  if (b.w01 != 0.f) mw += b.w01 * __half2float(reinterpret_cast<const __half*>(&prop_in[b.y0 * W + b.x0 + 1])[3]);
-  if (b.w10 != 0.f) mw += b.w10 * __half2float(reinterpret_cast<const __half*>(&prop_in[(b.y0 + 1) * W + b.x0])[3]);
-  if (b.w11 != 0.f) mw += b.w11 * __half2float(reinterpret_cast<const __half*>(&prop_in[(b.y0 + 1) * W + b.x0 + 1])[3]);
+  if (b.w00 != 0.f) mask_acc<S>(mw, b.w00, S::mask_at(prop_in, b.y0 * W + b.x0));
+  if (b.w01 != 0.f) mask_acc<S>(mw, b.w01, S::mask_at(prop_in, b.y0 * W + b.x0 + 1));
+  if (b.w10 != 0.f) mask_acc<S>(mw, b.w10, S::mask_at(prop_in, (b.y0 + 1) * W + b.x0));
+  if (b.w11 != 0.f) mask_acc<S>(mw, b.w11, S::mask_at(prop_in, (b.y0 + 1) * W + b.x0 + 1));
   const float mv = mw > 0.1f ? 1.f : 0.f;
-  const uint2 cu = cur[idx];
-  const float2 c01 = __half22float2(*reinterpret_cast<const __half2*>(&cu.x));
-  const float2 c23 = __half22float2(*reinterpret_cast<const __half2*>(&cu.y));
+  const typename S::Pix cu = cur[idx];
+  const float2 c01 = S::rg(cu);
+  const float2 c23 = S::bm(cu);
   const float mcur = c23.y;
   const float u = (mcur * valid * (1.f - mv)) > 0.1f ? 1.f : 0.f;
   const float mnew = (mcur * (1.f - valid * (1.f - mv))) > 0.1f ? 1.f : 0.f;
   const float r = u * wr + (1.f - u) * c01.x, g = u * wg + (1.f - u) * c01.y, bb = u * wb + (1.f - u) * c23.x;
-  uint2 o;
-  *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(r, g);
-  *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(bb, mnew);
-  prop_out[idx] = o;
+  prop_out[idx] = S::make(r, g, bb, mnew);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -112,59 +182,61 @@ __global__ void imgprop_step(const uint2* __restrict__ cur, const uint2* __restr
 // previous step (current pixel, both flows, the fb-consistency test, the sampling positions) is fetched for step
 // s+1 before the barrier of step s, so the serial chain per step is one barrier + one gather from L2.
 // ------------------------------------------------------------------------------------------------
+template <class S>
 struct PropPre {        // the step-independent half of one pixel's work
   int pix;              // pixel index in the frame, -1: nothing to do
   int near;             // nearest texel index of the propagated frame or -1
   int x0, y0;
   float w00, w01, w10, w11;
   float valid;
-  uint2 cur;
+  typename S::Pix cur;
 };
 
-__device__ __forceinline__ PropPre prop_pre(const uint2* __restrict__ cur, const __half2* __restrict__ flow_prop,
-                                            const __half2* __restrict__ flow_check, int pix, int H, int W, bool cur_is_input) {
-  PropPre r;
+template <class S>
+__device__ __forceinline__ PropPre<S> prop_pre(const typename S::Pix* __restrict__ cur,
+                                               const typename S::Flow* __restrict__ flow_prop,
+                                               const typename S::Flow* __restrict__ flow_check, int pix, int H, int W,
+                                               bool cur_is_input) {
+  PropPre<S> r;
   r.pix = pix;
   r.near = -1;
   r.cur = cur_is_input ? __ldg(&cur[pix]) : __ldcg(&cur[pix]);
-  const float mcur = __half2float(reinterpret_cast<const __half*>(&r.cur)[3]);
+  const float mcur = S::mask_of(r.cur);
   r.valid = 0.f; r.x0 = r.y0 = 0; r.w00 = r.w01 = r.w10 = r.w11 = 0.f;
   if (mcur == 0.f) { r.near = -2; return r; }          // -2: pass-through pixel
   const int x = pix % W, y = pix / W;
-  const float2 fp = __half22float2(__ldg(&flow_prop[pix]));
+  const float2 fp = S::flow(__ldg(&flow_prop[pix]));
   const float sx = sample_coord((float)x + fp.x, W), sy = sample_coord((float)y + fp.y, H);
   const Bilin b = bilin_setup(sx, sy, W, H);
-  r.valid = fb_valid(fp, sample_flow2(flow_check, b, W));
+  r.valid = fb_valid_of<S>(fp, flow_check, b, W);
   const int nx = (int)nearbyintf(sx), ny = (int)nearbyintf(sy);
   if (nx >= 0 && nx < W && ny >= 0 && ny < H) r.near = ny * W + nx;
   r.x0 = b.x0; r.y0 = b.y0; r.w00 = b.w00; r.w01 = b.w01; r.w10 = b.w10; r.w11 = b.w11;
   return r;
 }
 
-__device__ __forceinline__ uint2 prop_post(const PropPre& r, const uint2* prop_in, int W) {
+template <class S>
+__device__ __forceinline__ typename S::Pix prop_post(const PropPre<S>& r, const typename S::Pix* prop_in, int W) {
   float wr = 0.f, wg = 0.f, wb = 0.f;
   if (r.near >= 0) {
-    const uint2 t = __ldcg(&prop_in[r.near]);
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x));
-    const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
+    const typename S::Pix t = __ldcg(&prop_in[r.near]);
+    const float2 a = S::rg(t);
+    const float2 c = S::bm(t);
     wr = a.x; wg = a.y; wb = c.x;
   }
   float mw = 0.f;
-  auto mk = [&](int i) { const uint2 t = __ldcg(&prop_in[i]); return __half2float(reinterpret_cast<const __half*>(&t)[3]); };
-  if (r.w00 != 0.f) mw += r.w00 * mk(r.y0 * W + r.x0);
-  if (r.w01 != 0.f) mw += r.w01 * mk(r.y0 * W + r.x0 + 1);
-  if (r.w10 != 0.f) mw += r.w10 * mk((r.y0 + 1) * W + r.x0);
-  if (r.w11 != 0.f) mw += r.w11 * mk((r.y0 + 1) * W + r.x0 + 1);
+  auto mk = [&](int i) { return S::mask_of(__ldcg(&prop_in[i])); };
+  if (r.w00 != 0.f) mask_acc<S>(mw, r.w00, mk(r.y0 * W + r.x0));
+  if (r.w01 != 0.f) mask_acc<S>(mw, r.w01, mk(r.y0 * W + r.x0 + 1));
+  if (r.w10 != 0.f) mask_acc<S>(mw, r.w10, mk((r.y0 + 1) * W + r.x0));
+  if (r.w11 != 0.f) mask_acc<S>(mw, r.w11, mk((r.y0 + 1) * W + r.x0 + 1));
   const float mv = mw > 0.1f ? 1.f : 0.f;
-  const float2 c01 = __half22float2(*reinterpret_cast<const __half2*>(&r.cur.x));
-  const float2 c23 = __half22float2(*reinterpret_cast<const __half2*>(&r.cur.y));
+  const float2 c01 = S::rg(r.cur);
+  const float2 c23 = S::bm(r.cur);
   const float mcur = c23.y;
   const float u = (mcur * r.valid * (1.f - mv)) > 0.1f ? 1.f : 0.f;
   const float mnew = (mcur * (1.f - r.valid * (1.f - mv))) > 0.1f ? 1.f : 0.f;
-  uint2 o;
-  *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(u * wr + (1.f - u) * c01.x, u * wg + (1.f - u) * c01.y);
-  *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(u * wb + (1.f - u) * c23.x, mnew);
-  return o;
+  return S::make(u * wr + (1.f - u) * c01.x, u * wg + (1.f - u) * c01.y, u * wb + (1.f - u) * c23.x, mnew);
 }
 
 // bbox = {x0, y0, x1, y1} (inclusive) of mask > 0 over all frames; initialised to {W, H, -1, -1}
@@ -185,17 +257,20 @@ __global__ void mask_bbox(const float* __restrict__ masks, long long total, int 
   }
 }
 
-__global__ void __launch_bounds__(256) imgprop_persistent(const uint2* __restrict__ in4, uint2* bwd, uint2* fwd,
-                                                          const __half2* __restrict__ ff, const __half2* __restrict__ fbk,
-                                                          int T, int H, int W, const int* __restrict__ bbox,
-                                                          unsigned int* counter) {
+template <class S>
+__global__ void __launch_bounds__(256) imgprop_persistent(const typename S::Pix* __restrict__ in4, typename S::Pix* bwd,
+                                                          typename S::Pix* fwd, const typename S::Flow* __restrict__ ff,
+                                                          const typename S::Flow* __restrict__ fbk, int T, int H, int W,
+                                                          const int* __restrict__ bbox, unsigned int* counter) {
+  using Pix = typename S::Pix;
+  using Flow = typename S::Flow;
   const int bx0 = bbox[0], by0 = bbox[1], bw = bbox[2] - bbox[0] + 1, bh = bbox[3] - bbox[1] + 1;
   if (bbox[2] < 0) return;                                  // no hole anywhere: outputs are the pre-copied inputs
   const int npix = bw * bh;
   const int nthreads = gridDim.x * blockDim.x, gtid = blockIdx.x * blockDim.x + threadIdx.x;
   const long long HW = (long long)H * W;
   const int steps = 2 * (T - 1);
-  auto bufs = [&](int s, const uint2*& cur, const uint2*& pin, uint2*& out, const __half2*& fprop, const __half2*& fchk) {
+  auto bufs = [&](int s, const Pix*& cur, const Pix*& pin, Pix*& out, const Flow*& fprop, const Flow*& fchk) {
     if (s < T - 1) {          // backward pass: idx = T-2 .. 0, prop flow = forward flow, check = backward flow
       const int idx = T - 2 - s;
       cur = in4 + idx * HW; pin = bwd + (idx + 1) * HW; out = bwd + idx * HW; fprop = ff + idx * HW; fchk = fbk + idx * HW;
@@ -205,14 +280,14 @@ __global__ void __launch_bounds__(256) imgprop_persistent(const uint2* __restric
     }
   };
   auto pixel_of = [&](int j) { return (by0 + j / bw) * W + bx0 + j % bw; };
-  const uint2 *cur, *pin;
-  uint2* out;
-  const __half2 *fprop, *fchk;
-  PropPre pre;
+  const Pix *cur, *pin;
+  Pix* out;
+  const Flow *fprop, *fchk;
+  PropPre<S> pre;
   pre.pix = -1;
   if (gtid < npix) {
     bufs(0, cur, pin, out, fprop, fchk);
-    pre = prop_pre(cur, fprop, fchk, pixel_of(gtid), H, W, true);
+    pre = prop_pre<S>(cur, fprop, fchk, pixel_of(gtid), H, W, true);
   }
   for (int s = 0; s < steps; ++s) {
     bufs(s, cur, pin, out, fprop, fchk);
@@ -220,7 +295,7 @@ __global__ void __launch_bounds__(256) imgprop_persistent(const uint2* __restric
     // first pixel of this thread: its step-independent half was fetched before the previous barrier
     if (pre.pix >= 0) {
       if (pre.near != -2) {
-        const uint2 o = prop_post(pre, pin, W);
+        const Pix o = prop_post<S>(pre, pin, W);
         out[pre.pix] = o;
         if (s == T - 2) fwd[pre.pix] = o;                   // frame 0 of the forward pass is the backward result
       } else if (fwd_pass) {
@@ -230,9 +305,9 @@ __global__ void __launch_bounds__(256) imgprop_persistent(const uint2* __restric
       }
     }
     for (int j = gtid + nthreads; j < npix; j += nthreads) {   // holes larger than the grid: remaining pixels
-      const PropPre q = prop_pre(cur, fprop, fchk, pixel_of(j), H, W, !fwd_pass);
+      const PropPre<S> q = prop_pre<S>(cur, fprop, fchk, pixel_of(j), H, W, !fwd_pass);
       if (q.near != -2) {
-        const uint2 o = prop_post(q, pin, W);
+        const Pix o = prop_post<S>(q, pin, W);
         out[q.pix] = o;
         if (s == T - 2) fwd[q.pix] = o;
       } else if (fwd_pass) {
@@ -242,42 +317,41 @@ __global__ void __launch_bounds__(256) imgprop_persistent(const uint2* __restric
       }
     }
     if (s + 1 < steps && gtid < npix) {
-      const uint2 *c2, *p2;
-      uint2* o2;
-      const __half2 *f2, *k2;
+      const Pix *c2, *p2;
+      Pix* o2;
+      const Flow *f2, *k2;
       bufs(s + 1, c2, p2, o2, f2, k2);
       // in the forward pass `cur` is a backward-pass output of THIS thread (same pixel mapping), complete by now
-      pre = prop_pre(c2, f2, k2, pixel_of(gtid), H, W, s + 1 < T - 1);
+      pre = prop_pre<S>(c2, f2, k2, pixel_of(gtid), H, W, s + 1 < T - 1);
     }
     ppx::grid_barrier(counter, (unsigned)(s + 1) * gridDim.x);
   }
 }
 
-// frames [T,3,H,W] f32 (already multiplied by (1-mask) here) + masks -> [T][H][W][4] fp16
+// frames [T,3,H,W] f32 (already multiplied by (1-mask) here) + masks -> [T][H][W][4] fp16 / fp32
+template <class S>
 __global__ void imgprop_pack(const float* __restrict__ frames, const float* __restrict__ masks,
-                             uint2* __restrict__ dst, long long HW, long long total) {
+                             typename S::Pix* __restrict__ dst, long long HW, long long total) {
   long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const long long t = idx / HW, p = idx - t * HW;
   const float m = masks[idx];
   const float* f = frames + t * 3 * HW + p;
   const float k = 1.f - m;
-  uint2 o;
-  *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(f[0] * k, f[HW] * k);
-  *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(f[2 * HW] * k, m);
-  dst[idx] = o;
+  dst[idx] = S::make(f[0] * k, f[HW] * k, f[2 * HW] * k, m);
 }
 
 // updated = frames*(1-m) + prop*m ; updated mask = propagated mask   (propainter_inference.py:213-219)
-__global__ void imgprop_finish(const uint2* __restrict__ prop, const float* __restrict__ frames,
+template <class S>
+__global__ void imgprop_finish(const typename S::Pix* __restrict__ prop, const float* __restrict__ frames,
                                const float* __restrict__ masks, float* __restrict__ uf, float* __restrict__ um,
                                long long HW, long long total) {
   long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const long long t = idx / HW, p = idx - t * HW;
-  const uint2 v = prop[idx];
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-  const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+  const typename S::Pix v = prop[idx];
+  const float2 a = S::rg(v);
+  const float2 c = S::bm(v);
   const float m = masks[idx], k = 1.f - m;
   const float* f = frames + t * 3 * HW + p;
   float* o = uf + t * 3 * HW + p;
@@ -287,13 +361,14 @@ __global__ void imgprop_finish(const uint2* __restrict__ prop, const float* __re
   um[idx] = c.y;
 }
 
-// [n,2,H,W] f32 -> [n][H][W][2] fp16
-__global__ void flow_to_nhwc2(const float* __restrict__ src, __half2* __restrict__ dst, long long HW,
+// [n,2,H,W] f32 -> [n][H][W][2] fp16 / fp32
+template <class S>
+__global__ void flow_to_nhwc2(const float* __restrict__ src, typename S::Flow* __restrict__ dst, long long HW,
                               long long total) {
   long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const long long n = idx / HW, p = idx - n * HW;
-  dst[idx] = __floats2half2_rn(src[(n * 2) * HW + p], src[(n * 2 + 1) * HW + p]);
+  dst[idx] = S::make_flow(src[(n * 2) * HW + p], src[(n * 2 + 1) * HW + p]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -441,26 +516,27 @@ __global__ void downsample_mask4(const float* __restrict__ src, __half* __restri
   dst[idx * dst_cs + dst_co] = __float2half_rn(src[((long long)i * H + 4 * y) * W + 4 * x]);
 }
 
-}  // namespace
-
-int pp_k_imgprop_step(const __half* cur, const __half* prop_in, __half* prop_out, const __half* flow_prop,
-                      const __half* flow_check, int H, int W, cudaStream_t st) {
-  imgprop_step<<<nblocks((long long)H * W), TPB, 0, st>>>(
-      reinterpret_cast<const uint2*>(cur), reinterpret_cast<const uint2*>(prop_in), reinterpret_cast<uint2*>(prop_out),
-      reinterpret_cast<const __half2*>(flow_prop), reinterpret_cast<const __half2*>(flow_check), H, W);
+template <class S>
+int imgprop_step_launch(const void* cur, const void* prop_in, void* prop_out, const void* flow_prop,
+                        const void* flow_check, int H, int W, cudaStream_t st) {
+  using Pix = typename S::Pix;
+  using Flow = typename S::Flow;
+  imgprop_step<S><<<nblocks((long long)H * W), TPB, 0, st>>>(
+      static_cast<const Pix*>(cur), static_cast<const Pix*>(prop_in), static_cast<Pix*>(prop_out),
+      static_cast<const Flow*>(flow_prop), static_cast<const Flow*>(flow_check), H, W);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
 
-// bwd / fwd must hold copies of in4; scratch = 8 ints (bbox[4], barrier counter, pad)
-int pp_k_imgprop_run(const __half* in4, __half* bwd, __half* fwd, const __half* ff, const __half* fbk,
-                     const float* masks, int T, int H, int W, int* scratch, cudaStream_t st) {
-  static int grid_max = 0;
+template <class S>
+int imgprop_run(const void* in4, void* bwd, void* fwd, const void* ff, const void* fbk, const float* masks, int T,
+                int H, int W, int* scratch, cudaStream_t st) {
+  static int grid_max = 0;      // one per storage type: the fp32 kernel has its own register footprint
   if (grid_max == 0) {
     int dev = 0, sms = 0, per_sm = 0;
     PP_CUDA_CHECK(cudaGetDevice(&dev));
     PP_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PP_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, imgprop_persistent, 256, 0));
+    PP_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, imgprop_persistent<S>, 256, 0));
     PP_REQUIRE(per_sm >= 1, "imgprop: persistent kernel does not fit an SM");
     grid_max = sms * (per_sm < 2 ? per_sm : 2);
   }
@@ -470,40 +546,94 @@ int pp_k_imgprop_run(const __half* in4, __half* bwd, __half* fwd, const __half* 
   const long long want = (total + 256 * 16 - 1) / (256 * 16);
   mask_bbox<<<(int)(want < 1184 ? want : 1184), 256, 0, st>>>(masks, total, H * W, W, scratch);
   PP_CUDA_CHECK(cudaGetLastError());
-  const uint2* a0 = reinterpret_cast<const uint2*>(in4);
-  uint2* a1 = reinterpret_cast<uint2*>(bwd);
-  uint2* a2 = reinterpret_cast<uint2*>(fwd);
-  const __half2* a3 = reinterpret_cast<const __half2*>(ff);
-  const __half2* a4 = reinterpret_cast<const __half2*>(fbk);
+  using Pix = typename S::Pix;
+  using Flow = typename S::Flow;
+  const Pix* a0 = static_cast<const Pix*>(in4);
+  Pix* a1 = static_cast<Pix*>(bwd);
+  Pix* a2 = static_cast<Pix*>(fwd);
+  const Flow* a3 = static_cast<const Flow*>(ff);
+  const Flow* a4 = static_cast<const Flow*>(fbk);
   const int* a8 = scratch;
   unsigned int* a9 = reinterpret_cast<unsigned int*>(scratch + 4);
   void* args[] = {&a0, &a1, &a2, &a3, &a4, &T, &H, &W, &a8, &a9};
-  PP_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)imgprop_persistent, dim3(grid_max), dim3(256), args, 0, st));
+  PP_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)imgprop_persistent<S>, dim3(grid_max), dim3(256), args, 0, st));
   return PP_OK;
 }
 
-int pp_k_imgprop_pack(const float* frames, const float* masks, __half* dst, int T, int H, int W, cudaStream_t st) {
+template <class S>
+int imgprop_pack_launch(const float* frames, const float* masks, void* dst, int T, int H, int W, cudaStream_t st) {
   const long long HW = (long long)H * W, total = HW * T;
-  imgprop_pack<<<nblocks(total), TPB, 0, st>>>(frames, masks, reinterpret_cast<uint2*>(dst), HW, total);
+  imgprop_pack<S><<<nblocks(total), TPB, 0, st>>>(frames, masks, static_cast<typename S::Pix*>(dst), HW, total);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
+}
+
+template <class S>
+int imgprop_finish_launch(const void* prop, const float* frames, const float* masks, float* upd_frames,
+                          float* upd_masks, int T, int H, int W, cudaStream_t st) {
+  const long long HW = (long long)H * W, total = HW * T;
+  imgprop_finish<S><<<nblocks(total), TPB, 0, st>>>(static_cast<const typename S::Pix*>(prop), frames, masks,
+                                                    upd_frames, upd_masks, HW, total);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+template <class S>
+int flow_to_nhwc2_launch(const float* src, void* dst, int n, int H, int W, cudaStream_t st) {
+  const long long HW = (long long)H * W, total = HW * n;
+  if (total == 0) return PP_OK;
+  flow_to_nhwc2<S><<<nblocks(total), TPB, 0, st>>>(src, static_cast<typename S::Flow*>(dst), HW, total);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+}  // namespace
+
+int pp_k_imgprop_step(const __half* cur, const __half* prop_in, __half* prop_out, const __half* flow_prop,
+                      const __half* flow_check, int H, int W, cudaStream_t st) {
+  return imgprop_step_launch<ImgF16>(cur, prop_in, prop_out, flow_prop, flow_check, H, W, st);
+}
+
+int pp_k_imgprop_step_f32(const float* cur, const float* prop_in, float* prop_out, const float* flow_prop,
+                          const float* flow_check, int H, int W, cudaStream_t st) {
+  return imgprop_step_launch<ImgF32>(cur, prop_in, prop_out, flow_prop, flow_check, H, W, st);
+}
+
+// bwd / fwd must hold copies of in4; scratch = 8 ints (bbox[4], barrier counter, pad)
+int pp_k_imgprop_run(const __half* in4, __half* bwd, __half* fwd, const __half* ff, const __half* fbk,
+                     const float* masks, int T, int H, int W, int* scratch, cudaStream_t st) {
+  return imgprop_run<ImgF16>(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st);
+}
+
+int pp_k_imgprop_run_f32(const float* in4, float* bwd, float* fwd, const float* ff, const float* fbk,
+                         const float* masks, int T, int H, int W, int* scratch, cudaStream_t st) {
+  return imgprop_run<ImgF32>(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st);
+}
+
+int pp_k_imgprop_pack(const float* frames, const float* masks, __half* dst, int T, int H, int W, cudaStream_t st) {
+  return imgprop_pack_launch<ImgF16>(frames, masks, dst, T, H, W, st);
+}
+
+int pp_k_imgprop_pack_f32(const float* frames, const float* masks, float* dst, int T, int H, int W, cudaStream_t st) {
+  return imgprop_pack_launch<ImgF32>(frames, masks, dst, T, H, W, st);
 }
 
 int pp_k_imgprop_finish(const __half* prop, const float* frames, const float* masks, float* upd_frames,
                         float* upd_masks, int T, int H, int W, cudaStream_t st) {
-  const long long HW = (long long)H * W, total = HW * T;
-  imgprop_finish<<<nblocks(total), TPB, 0, st>>>(reinterpret_cast<const uint2*>(prop), frames, masks, upd_frames,
-                                                 upd_masks, HW, total);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
+  return imgprop_finish_launch<ImgF16>(prop, frames, masks, upd_frames, upd_masks, T, H, W, st);
+}
+
+int pp_k_imgprop_finish_f32(const float* prop, const float* frames, const float* masks, float* upd_frames,
+                            float* upd_masks, int T, int H, int W, cudaStream_t st) {
+  return imgprop_finish_launch<ImgF32>(prop, frames, masks, upd_frames, upd_masks, T, H, W, st);
 }
 
 int pp_k_flow_to_nhwc2(const float* src, __half* dst, int n, int H, int W, cudaStream_t st) {
-  const long long HW = (long long)H * W, total = HW * n;
-  if (total == 0) return PP_OK;
-  flow_to_nhwc2<<<nblocks(total), TPB, 0, st>>>(src, reinterpret_cast<__half2*>(dst), HW, total);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
+  return flow_to_nhwc2_launch<ImgF16>(src, dst, n, H, W, st);
+}
+
+int pp_k_flow_to_nhwc2_f32(const float* src, float* dst, int n, int H, int W, cudaStream_t st) {
+  return flow_to_nhwc2_launch<ImgF32>(src, dst, n, H, W, st);
 }
 
 int pp_k_rfc_pack_input(const float* flows, const float* masks, __half* dst, long long dst_tstride_pix, int T, int H,

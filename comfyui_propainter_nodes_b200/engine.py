@@ -43,6 +43,7 @@ _SIGNATURES = {
     "pp_flow_complete": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
     "pp_flow_complete_dist": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _I, _I, _VP]),
     "pp_image_propagate": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
+    "pp_image_propagate_fp32": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
     "pp_gen_begin": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
     "pp_gen_begin_subset": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, ctypes.c_char_p, _VP]),
     "pp_gen_window": (_I, [_VP, ctypes.POINTER(_I), _I, _I, _VP, _VP]),
@@ -67,6 +68,7 @@ _SIGNATURES = {
     "pp_op_corr_lookup_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
     "pp_op_convex_upsample": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "pp_op_imgprop_step": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP]),
+    "pp_op_imgprop_step_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP]),
     "pp_op_attention": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
 }
 
@@ -521,12 +523,16 @@ class Engine:
                                                    _ptr(of), _ptr(ob), int(team_first), int(team_size), self._stream()))
         return of, ob
 
-    def image_propagate(self, frames, masks, flows_f, flows_b):
+    def image_propagate(self, frames, masks, flows_f, flows_b, fp32: bool = False):
+        """frames [T,3,H,W], masks [T,1,H,W], completed flows [T-1,2,H,W] -> (updated frames, updated masks).
+        fp32=False stores frames and flows in fp16 inside the propagation; fp32=True keeps them in fp32
+        (pp_image_propagate_fp32), what the node runs for fp16="disable"."""
         frames, masks, flows_f, flows_b = map(self._f32, (frames, masks, flows_f, flows_b))
         T, _, H, W = frames.shape
         uf, um = torch.empty_like(frames), torch.empty_like(masks)
-        self._check(self.lib.pp_image_propagate(self.h, _ptr(frames), _ptr(masks), _ptr(flows_f), _ptr(flows_b), T, H, W,
-                                                _ptr(uf), _ptr(um), self._stream()))
+        fn = self.lib.pp_image_propagate_fp32 if fp32 else self.lib.pp_image_propagate
+        self._check(fn(self.h, _ptr(frames), _ptr(masks), _ptr(flows_f), _ptr(flows_b), T, H, W, _ptr(uf), _ptr(um),
+                       self._stream()))
         return uf, um
 
     def gen_begin(self, updated_frames, masks_dilated, updated_masks, flows_f, flows_b, frames_needed=None):
@@ -822,6 +828,14 @@ class Engine:
         out = torch.empty_like(cur4)
         self._check(self.lib.pp_op_imgprop_step(self.h, _ptr(cur4), _ptr(prop4), _ptr(out), _ptr(flow_prop),
                                                 _ptr(flow_check), H, W, self._stream()))
+        return out
+
+    def op_imgprop_step_f32(self, cur4, prop4, flow_prop, flow_check):
+        """One fp32 propagation step: cur4 / prop4 float32 [H,W,4] (r, g, b, mask), flows float32 [H,W,2]."""
+        H, W, _ = cur4.shape
+        out = torch.empty_like(cur4)
+        self._check(self.lib.pp_op_imgprop_step_f32(self.h, _ptr(cur4), _ptr(prop4), _ptr(out), _ptr(flow_prop),
+                                                    _ptr(flow_check), H, W, self._stream()))
         return out
 
     def op_attention(self, qkv, pkv, win_flags, t, gh, gw, n_pool, parity):

@@ -12,8 +12,9 @@ exactly where the reference calls its PyTorch modules:
 
 Tensors keep the reference layouts ([1,T,C,H,W]).  RAFT follows the ``fp16`` switch: "enable" runs it with fp16
 activations and fp32 accumulation, "disable" at fp32 accuracy (fp32 activations, 3xTF32 GEMMs), like the reference,
-which always runs RAFT in fp32.  Flow completion and the generator compute in fp16 with fp32 accumulation in both
-modes (there the switch only selects the dtype of the tensors handed back).
+which always runs RAFT in fp32.  Image propagation follows it too: "disable" keeps frames, masks and flows in fp32
+(pp_image_propagate_fp32), "enable" stores them in fp16.  Flow completion and the generator compute in fp16 with fp32
+accumulation in both modes (there the switch only selects the dtype of the tensors handed back).
 """
 from __future__ import annotations
 
@@ -94,22 +95,26 @@ def complete_flow(recurrent_flow_model, flows_tuple, flow_masks: torch.Tensor, s
 
 def image_propagation(inpaint_model, frames: torch.Tensor, masks_dilated: torch.Tensor, prediction_flows,
                       config: ProPainterConfig):
-    """Non-learnable pixel propagation -> (updated_frames [1,T,3,H,W], updated_masks [1,T,1,H,W])."""
+    """Non-learnable pixel propagation -> (updated_frames [1,T,3,H,W], updated_masks [1,T,1,H,W]).
+
+    fp16="disable" keeps frames and flows in fp32 through the propagation (its decisions are discrete: an fp16 flow
+    moves whole pixels); "enable" stores them in fp16."""
     eng = inpaint_model.engine
     fr, md = frames[0], masks_dilated[0]
     ff, fb = prediction_flows[0][0], prediction_flows[1][0]
     dt = frames.dtype
     T = config.video_length
+    fp32 = not config.use_half
     sub = min(100, config.subvideo_length)
     if T <= sub:
-        uf, um = eng.image_propagate(fr, md, ff, fb)
+        uf, um = eng.image_propagate(fr, md, ff, fb, fp32=fp32)
     else:
         pad = 10
         lf, lm = [], []
         for f in range(0, T, sub):
             s, e = max(0, f - pad), min(T, f + sub + pad)
             ps, pe = f - s, e - min(T, f + sub)
-            a, b = eng.image_propagate(fr[s:e], md[s:e], ff[s:e - 1], fb[s:e - 1])
+            a, b = eng.image_propagate(fr[s:e], md[s:e], ff[s:e - 1], fb[s:e - 1], fp32=fp32)
             lf.append(a[ps:e - s - pe])
             lm.append(b[ps:e - s - pe])
         uf, um = torch.cat(lf, 0), torch.cat(lm, 0)

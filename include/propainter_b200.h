@@ -9,7 +9,7 @@
  *                                    (RAFT_bi.forward, model/modules/flow_comp_raft.py:39-58)
  *   pp_flow_complete       replaces  forward_bidirect_flow + combine_flow     propainter_inference.py:123-150
  *                                    (model/recurrent_flow_completion.py:356-400)
- *   pp_image_propagate     replaces  img_propagation + blend                  propainter_inference.py:186-219
+ *   pp_image_propagate[_fp32] replaces img_propagation + blend               propainter_inference.py:186-219
  *                                    (model/propainter.py:350-356, 118-231)
  *   pp_gen_begin/window    replace   inpaint_model(selected_imgs, ...)        propainter_inference.py:272-281
  *                                    (InpaintGenerator.forward, model/propainter.py:358-453)
@@ -91,6 +91,13 @@ PP_API int pp_flow_complete_dist(pp_handle h, const float* flows_f, const float*
 PP_API int pp_image_propagate(pp_handle h, const float* frames, const float* masks, const float* flows_f,
                        const float* flows_b, int T, int H, int W, float* updated_frames, float* updated_masks,
                        void* stream);
+/* The same at fp32 accuracy (the node's fp16="disable"): frames, masks and flows stay fp32 through the 2(T-1) steps,
+ * and the bilinear weights and sums and the forward-backward test are rounded as torch evaluates them in fp32 on the
+ * CPU, so the discrete decisions (fb validity, the 0.1 mask threshold, the nearest-pixel warp) are the ones the
+ * reference takes there.  pp_image_propagate stores fp16 frames and flows. */
+PP_API int pp_image_propagate_fp32(pp_handle h, const float* frames, const float* masks, const float* flows_f,
+                                   const float* flows_b, int T, int H, int W, float* updated_frames,
+                                   float* updated_masks, void* stream);
 /* Generator session over one clip: encodes all T frames once. */
 PP_API int pp_gen_begin(pp_handle h, const float* updated_frames, const float* masks_dilated, const float* updated_masks,
                  const float* flows_f, const float* flows_b, int T, int H, int W, void* stream);
@@ -183,6 +190,10 @@ PP_API int pp_op_convex_upsample(pp_handle h, const float* coords1, const void* 
                                  int fp32, void* stream);
 PP_API int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* prop_in4_f16, void* prop_out4_f16,
                        const void* flow_prop_f16, const void* flow_check_f16, int H, int W, void* stream);
+/* One image-propagation step of pp_image_propagate_fp32: pixels float32 [H][W][4] (r, g, b, mask), flows float32
+ * [H][W][2]. */
+PP_API int pp_op_imgprop_step_f32(pp_handle h, const float* cur4, const float* prop_in4, float* prop_out4,
+                                  const float* flow_prop, const float* flow_check, int H, int W, void* stream);
 PP_API int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,
                     int t, int gh, int gw, int n_pool, int parity, void* stream);
 
