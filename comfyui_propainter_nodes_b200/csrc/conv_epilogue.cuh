@@ -8,10 +8,11 @@ namespace ppconv {
 
 // ACC (the split-tf32 epilogue): fp32-accurate tanh (pp_common.cuh) instead of the fast-math tanh.approx, whose error is
 // below the fp16 storage rounding but far above fp32's
-template <int ACT, bool ACC = false>
-__device__ __forceinline__ void act16_t(float (&v)[16], float slope) {
+// Works on any run of N values: 16 consecutive channels in conv_epilogue16, a fragment's 4 values in conv_gemm.cu.
+template <int ACT, bool ACC = false, int N>
+__device__ __forceinline__ void act16_t(float (&v)[N], float slope) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < N; ++i) {
     if (ACT == PP_ACT_RELU) v[i] = fmaxf(v[i], 0.f);
     else if (ACT == PP_ACT_LRELU) v[i] = v[i] > 0.f ? v[i] : v[i] * slope;
     else if (ACT == PP_ACT_SIGMOID) v[i] = ppx::sigmoidf_(v[i]);
@@ -19,9 +20,9 @@ __device__ __forceinline__ void act16_t(float (&v)[16], float slope) {
     else if (ACT == PP_ACT_GELU) v[i] = ppx::gelu_erf(v[i]);
   }
 }
-// one (uniform) branch per 16 values instead of one per value
-template <bool ACC = false>
-__device__ __forceinline__ void act16(float (&v)[16], int act, float slope) {
+// one (uniform) branch per N values instead of one per value
+template <bool ACC = false, int N>
+__device__ __forceinline__ void act16(float (&v)[N], int act, float slope) {
   switch (act) {
     case PP_ACT_RELU: act16_t<PP_ACT_RELU, ACC>(v, slope); break;
     case PP_ACT_LRELU: act16_t<PP_ACT_LRELU, ACC>(v, slope); break;
@@ -106,11 +107,10 @@ __device__ __forceinline__ void conv_epilogue_prefetch16(const PPConvParams& p, 
 
 // `raw`: 16 fp32 accumulators (tile columns ng0-n0 .. +15) of output pixel `mrow` (flattened N*OH*OW index),
 // group g, first channel ng0 (within the group; ng0 < Cout_g).  `epi`/`vec` are launch-uniform.
-// sm0 / sm1 (STD epilogue, fp16 output only): when non-null the 16 results go to these two 16-byte shared-memory slots
-// (a staging tile that a TMA store writes out) instead of global memory.
+// The PP_EPI_STD branch's operation order is repeated per value by conv_gemm.cu's fragment epilogue (gemm_epi4); keep
+// the two in step, the flat layers' results do not depend on which kernel ran them.
 __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uint32_t (&raw)[16], long long mrow, int g,
-                                                int ng0, int epi, bool vec, const EpiAux* pre = nullptr,
-                                                uint4* sm0 = nullptr, uint4* sm1 = nullptr) {
+                                                int ng0, int epi, bool vec, const EpiAux* pre = nullptr) {
     const int nvalid = min(16, p.Cout_g - ng0);
     float v[16];
 #pragma unroll
@@ -155,12 +155,6 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
           for (int i = 0; i < 16; ++i)
             if (i < nvalid) dst[i] = v[i];
         }
-      } else if (sm0 != nullptr) {
-        __align__(16) __half2 h[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-        *sm0 = reinterpret_cast<uint4*>(h)[0];
-        *sm1 = reinterpret_cast<uint4*>(h)[1];
       } else {
         store16(reinterpret_cast<__half*>(p.out) + o, nvalid, vec, v);
       }
@@ -337,8 +331,7 @@ __device__ __forceinline__ void drain_acc(const float (&acc)[N / 2], float* stg,
 // conv_epilogue16 (SPLIT: conv_epilogue16_split) on 16 staged accumulators.  EPI >= 0: the layer's epilogue kind, known
 // at compile time (only that branch of conv_epilogue16 is generated); -1: p.epi at run time.
 template <bool SPLIT = false, int EPI = -1>
-__device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const float* src, long long mrow, int g, int ng0,
-                                                    uint4* sm0, uint4* sm1) {
+__device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const float* src, long long mrow, int g, int ng0) {
   if constexpr (SPLIT) {
     float acc[16];
 #pragma unroll
@@ -355,7 +348,7 @@ __device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const
       raw[i] = __float_as_uint(v.x); raw[i + 1] = __float_as_uint(v.y);
       raw[i + 2] = __float_as_uint(v.z); raw[i + 3] = __float_as_uint(v.w);
     }
-    conv_epilogue16(p, raw, mrow, g, ng0, EPI >= 0 ? EPI : p.epi, p.vec_ok != 0, nullptr, sm0, sm1);
+    conv_epilogue16(p, raw, mrow, g, ng0, EPI >= 0 ? EPI : p.epi, p.vec_ok != 0, nullptr);
   }
 }
 

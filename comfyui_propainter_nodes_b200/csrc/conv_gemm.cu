@@ -1,0 +1,358 @@
+// Wide-tile wgmma GEMM for the flat layers (1x1 convolutions and linear layers) on sm_90a:
+//   out[M x Cout] = epilogue( A[M x Cin] * W[Cout x Cin]^T ),  A = the flattened N*H*W pixels of the input segments.
+//
+// The halo kernel's flat mode runs these with 256 x <=128 tiles and drains the accumulators through a shared-memory
+// staging tile 32 columns at a time (two named barriers per chunk, 32-byte per-thread global stores); the tensor cores
+// idle meanwhile.  Here:
+//   * tiles are 128 x 256 (MB = 1: each consumer warpgroup owns 64 rows x 256 columns, wgmma m64n256k16) or, for layers
+//     with Cout <= 128, 256 x 128 (MB = 2: two m64 blocks of 128 columns), 128 accumulator registers per thread either
+//     way.  Per 64-channel K chunk a stage holds the A rows (one 2-D TMA box per segment view, zero-filled past M and
+//     past the last segment's channels) and the pre-swizzled weight tile (cp.async.bulk), 48 KB in both shapes.
+//   * the epilogue runs on the wgmma fragments: bias, act1, scale, residual, act2 in the order of conv_epilogue16's
+//     PP_EPI_STD branch, fp16 into a 128B-swizzled staging tile from which one thread per warpgroup issues TMA stores
+//     (rows / columns past the tensor are clipped).  The stores drain while the next tile's main loop runs; the staging
+//     tile is only waited for (cp.async.bulk.wait_group.read) before it is written again.  A residual tile (the in-place
+//     transformer proj) is TMA-loaded into the staging tile, read and overwritten in place by the same threads.
+//     The tile's bias columns are copied to shared memory once per tile and act1 is a compile-time case, so the loop
+//     over the fragments is straight-line code: with a global bias load per fragment column and a runtime activation
+//     switch it took ~9.5 us of a 128 x 256 tile (measured on H100), more than the tile's main loop.
+//   * the stage ring keeps running across tiles, so the producer loads the next tile during the epilogue.  Tiles are
+//     ordered N-fastest: the CTAs in flight share their A rows in L2.
+// Warp roles (384 threads, one persistent CTA per SM): warpgroups 0-1 consumers, warp 8 producer (one elected thread
+// issues both loads of a stage), warps 9-11 idle (setmaxnreg works per warpgroup).
+#include <stdlib.h>
+#include <string.h>
+
+#include "conv_epilogue.cuh"
+#include "conv_igemm.cuh"
+
+namespace {
+
+constexpr int NUM_THREADS = 384;
+constexpr int NUM_CONSUMERS = 256;
+constexpr int WARP_PRODUCER = 8;
+constexpr int STAGE_BYTES = 48 * 1024;        // A [128*MB rows][128 B] + B [256/MB rows][128 B]
+constexpr int STAGES = 3;
+constexpr int OUT_BYTES = 64 * 1024;          // fp16 staging tile [256/MB / 64 panels][128*MB rows][128 B]
+constexpr int BIAS_BYTES = 2 * 256 * 4;       // the tile's bias columns, one copy per consumer warpgroup
+constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + OUT_BYTES + 1024 + BIAS_BYTES;   // alignment slack, barriers
+
+struct GemmParams {
+  PPConvParams c;
+  CUtensorMap tmap_a[PP_MAX_SEGS];
+  CUtensorMap tmap_out;   // [M][Cout] at out + out_coff, boxes of 64 columns x 64*MB rows (one warpgroup's rows)
+  CUtensorMap tmap_res;   // the same for the residual (aux0), when there is one
+  int m_tiles, n_tiles, chunks;
+  int debug;              // bit 0: skip the epilogue math/stores (PP_CONV_NOEPI=1, mainloop-only timing experiments)
+};
+
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, 0, 0}], [%2];" ::"r"(dst),
+      "l"(tmap), "r"(ppx::smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
+      "l"(tmap), "r"(ppx::smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+
+struct Smem {
+  uint8_t* stages;
+  uint8_t* out;
+  uint64_t *full, *empty, *res;   // res: one barrier per consumer warpgroup
+  float* bias;                    // [2][256]
+};
+__device__ __forceinline__ Smem gemm_smem() {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = ppx::smem_u32(smem_raw);
+  uint8_t* base = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  Smem m;
+  m.stages = base;
+  m.out = base + STAGES * STAGE_BYTES;
+  m.full = reinterpret_cast<uint64_t*>(m.out + OUT_BYTES);
+  m.empty = m.full + STAGES;
+  m.res = m.empty + STAGES;
+  m.bias = reinterpret_cast<float*>(m.out + OUT_BYTES + 1024);
+  return m;
+}
+
+// 4 accumulators of one fragment column pair (rows r and r + 8, columns c, c + 1) through the PP_EPI_STD epilogue, in
+// conv_epilogue16's operation order.  ACT1: p.act1 (dispatched once per tile, so the loop over the fragments has no
+// indirect branch); act2 is PP_ACT_NONE on every flat layer but is still applied when set.
+template <int ACT1>
+__device__ __forceinline__ void gemm_epi4(float (&v)[4], bool has_bias, const float2& bias, float scale, bool has_res,
+                                          const float (&res)[4], int act2, float slope) {
+  if (has_bias) {
+    v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
+  }
+  ppconv::act16_t<ACT1>(v, slope);
+  if (scale != 1.f) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] *= scale;
+  }
+  if (has_res) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] += res[i];
+  }
+  if (act2 != PP_ACT_NONE) ppconv::act16(v, act2, slope);
+}
+
+// The fragment epilogue of one warpgroup into its rows of the staging tile `so`.  Every column of the tile is written
+// (the staging tile has room for all of them; columns past Cout_g are never stored), so the loop is straight-line code
+// whose shared-memory loads and stores the compiler can batch.
+template <int MB, int BN, int ACT1>
+__device__ __forceinline__ void gemm_epilogue(const PPConvParams& p, const float (&acc)[MB][BN / 2], uint8_t* so,
+                                              const float* bs, bool has_res, int t128) {
+  constexpr int PANEL = 128 * MB * 128;
+  const bool has_bias = p.bias != nullptr;
+  const float scale = p.scale, slope = p.slope;
+  const int act2 = p.act2;
+  // fragment of m64nNk16: register 4j + i of thread t holds row 16 * (t / 32) + (t % 32) / 4 + 8 * (i / 2), column
+  // 8j + 2 * (t % 4) + i % 2
+  const int fr = 16 * (t128 >> 5) + ((t128 & 31) >> 2), fc = 2 * (t128 & 3);
+#pragma unroll
+  for (int b = 0; b < MB; ++b) {
+    const int r = 64 * b + fr;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = 8 * j + fc;
+      // 128B swizzle: the 16-byte unit (col % 64) / 8 of row r sits at unit index XOR (r & 7); (r + 8) & 7 == r & 7
+      const int off = (col >> 6) * PANEL + r * 128 + (((((col & 63) >> 3) ^ (r & 7))) << 4) + (col & 7) * 2;
+      __half2* lo = reinterpret_cast<__half2*>(so + off);
+      __half2* hi = reinterpret_cast<__half2*>(so + off + 8 * 128);
+      const float2 bias = *reinterpret_cast<const float2*>(bs + col);
+      float v[4] = {acc[b][4 * j], acc[b][4 * j + 1], acc[b][4 * j + 2], acc[b][4 * j + 3]};
+      float res[4] = {0.f, 0.f, 0.f, 0.f};
+      if (has_res) {
+        const float2 r0 = __half22float2(*lo), r1 = __half22float2(*hi);
+        res[0] = r0.x; res[1] = r0.y; res[2] = r1.x; res[3] = r1.y;
+      }
+      gemm_epi4<ACT1>(v, has_bias, bias, scale, has_res, res, act2, slope);
+      *lo = __floats2half2_rn(v[0], v[1]);
+      *hi = __floats2half2_rn(v[2], v[3]);
+    }
+  }
+}
+
+// One tile of one consumer warpgroup: main loop into acc[MB][BN / 2], then the fragment epilogue into the staging tile
+// and this warpgroup's TMA stores.  The ring position (s, ph) runs on across tiles.
+template <int MB, int BN>
+__device__ __forceinline__ void gemm_tile(const GemmParams& h, const Smem& m, int tile, int& s, uint32_t& ph, uint32_t& rph,
+                                          int wg, int t128) {
+  using namespace ppx;
+  const PPConvParams& p = h.c;
+  constexpr int A_BYTES = 128 * MB * 128;
+  constexpr int WG_ROWS = 64 * MB;
+  constexpr int PANEL = 128 * MB * 128;        // one 64-column panel of the staging tile
+  const int n0 = (tile % h.n_tiles) * BN;
+  const int m0 = (tile / h.n_tiles) * (128 * MB);
+  float acc[MB][BN / 2];
+  int prev = -1;
+  for (int c = 0; c < h.chunks; ++c) {
+    mbar_wait(&m.full[s], ph);
+    const uint32_t a = smem_u32(m.stages + s * STAGE_BYTES);
+    uint64_t adesc[MB];
+#pragma unroll
+    for (int b = 0; b < MB; ++b) adesc[b] = gmma_desc_sw128_kmajor(a + (wg * MB + b) * 64 * 128);
+    const uint64_t bdesc = gmma_desc_sw128_kmajor(a + A_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int b = 0; b < MB; ++b) wgmma_f16<BN>(acc[b], adesc[b] + 2 * k, bdesc + 2 * k, (c | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0) mbar_arrive(&m.empty[prev]);
+    prev = s;
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int b = 0; b < MB; ++b) wgmma_fence_acc(acc[b]);
+  mbar_arrive(&m.empty[prev]);
+  if (h.debug & 1) return;
+
+  // ---- epilogue: this warpgroup's rows [wg * WG_ROWS, +WG_ROWS) of every panel of the staging tile
+  const int bar_id = 2 + wg, row0 = m0 + wg * WG_ROWS;
+  const int npanel = (min(BN, p.Cout_g - n0) + 63) / 64;
+  uint8_t* so = m.out + wg * WG_ROWS * 128;
+  const bool issuer = t128 == 0;
+  // the tile's bias columns (one coalesced load per thread instead of a dependent load per fragment column); the
+  // previous tile's readers of this copy have passed its last named barrier
+  float* bs = m.bias + wg * 256;
+  {
+    const int c0 = 2 * t128, n = n0 + c0;
+    float2 bv = make_float2(0.f, 0.f);
+    if (p.bias != nullptr && c0 < BN) {
+      if (n < p.Cout_g) bv.x = __ldg(p.bias + n);
+      if (n + 1 < p.Cout_g) bv.y = __ldg(p.bias + n + 1);
+    }
+    if (c0 < BN) *reinterpret_cast<float2*>(bs + c0) = bv;
+  }
+  if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
+  named_bar(bar_id, 128);
+  const bool has_res = p.aux0 != nullptr;
+  if (has_res) {
+    if (issuer) {
+      mbar_arrive_expect_tx(&m.res[wg], (uint32_t)(npanel * WG_ROWS * 128));
+      for (int pnl = 0; pnl < npanel; ++pnl) tma_load_2d(smem_u32(so + pnl * PANEL), &h.tmap_res, n0 + pnl * 64, row0, &m.res[wg]);
+    }
+    mbar_wait(&m.res[wg], rph);
+    rph ^= 1;
+  }
+  switch (p.act1) {
+    case PP_ACT_RELU: gemm_epilogue<MB, BN, PP_ACT_RELU>(p, acc, so, bs, has_res, t128); break;
+    case PP_ACT_LRELU: gemm_epilogue<MB, BN, PP_ACT_LRELU>(p, acc, so, bs, has_res, t128); break;
+    case PP_ACT_SIGMOID: gemm_epilogue<MB, BN, PP_ACT_SIGMOID>(p, acc, so, bs, has_res, t128); break;
+    case PP_ACT_TANH: gemm_epilogue<MB, BN, PP_ACT_TANH>(p, acc, so, bs, has_res, t128); break;
+    case PP_ACT_GELU: gemm_epilogue<MB, BN, PP_ACT_GELU>(p, acc, so, bs, has_res, t128); break;
+    default: gemm_epilogue<MB, BN, PP_ACT_NONE>(p, acc, so, bs, has_res, t128); break;
+  }
+  fence_proxy_async();           // generic-proxy smem writes -> visible to the TMA store
+  named_bar(bar_id, 128);
+  if (issuer) {
+    for (int pnl = 0; pnl < npanel; ++pnl) tma_store_2d(&h.tmap_out, smem_u32(so + pnl * PANEL), n0 + pnl * 64, row0);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+  }
+}
+
+template <int MB>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_constant__ GemmParams h) {
+  using namespace ppx;
+  constexpr int BN = 256 / MB;
+  constexpr int A_BYTES = 128 * MB * 128;
+  const Smem m = gemm_smem();
+  const PPConvParams& p = h.c;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int total_tiles = h.m_tiles * h.n_tiles;
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&m.full[s], 1); mbar_init(&m.empty[s], NUM_CONSUMERS); }
+    mbar_init(&m.res[0], 1);
+    mbar_init(&m.res[1], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  // as in the halo kernel: the producer warpgroup gives its registers to the accumulator holders
+  if (warp < 8) setmaxnreg_inc<232>();
+  else setmaxnreg_dec<40>();
+  if (warp < 8) {
+    const int wg = tid >> 7, t128 = tid & 127;
+    int s = 0;
+    uint32_t ph = 0, rph = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) gemm_tile<MB, BN>(h, m, tile, s, ph, rph, wg, t128);
+    if (t128 == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // this warpgroup's stores complete
+  } else if (warp == WARP_PRODUCER) {
+    if (elect_one()) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int n0 = (tile % h.n_tiles) * BN;
+        const int m0 = (tile / h.n_tiles) * (128 * MB);
+        // columns >= bnt of the last N tile keep stale weights: computed, never stored
+        const uint32_t b_bytes = (uint32_t)(min(BN, p.Cout_g_pad - n0) * 128);
+        for (int c = 0; c < h.chunks; ++c) {
+          const int ci = c * 64;
+          int q = 0;
+#pragma unroll
+          for (int k = 1; k < PP_MAX_SEGS; ++k)
+            if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
+          mbar_wait(&m.empty[s], ph ^ 1);
+          mbar_arrive_expect_tx(&m.full[s], (uint32_t)A_BYTES + b_bytes);
+          const uint32_t dst = smem_u32(m.stages + s * STAGE_BYTES);
+          tma_load_4d(dst, &h.tmap_a[q], ci - p.seg[q].cbegin, m0, &m.full[s]);
+          bulk_g2s(dst + A_BYTES, p.wpacked + ((long long)c * p.Cout_g_pad + n0) * 64, b_bytes, &m.full[s]);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  }
+}
+
+int gemm_num_sms() {
+  static int num_sms = 0;
+  if (num_sms == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+      return 0;
+  }
+  return num_sms;
+}
+
+// MB (m64 blocks per consumer warpgroup) of a layer: 256 x 128 tiles when all output channels fit one 128-wide tile
+int gemm_mb(const PPConvParams& p) { return p.Cout_g_pad <= 128 && p.M_total >= 256 ? 2 : 1; }
+
+long long gemm_tiles(const PPConvParams& p, int mb) {
+  return pp_ceil_div64(p.M_total, 128 * mb) * pp_ceil_div(p.Cout_g_pad, 256 / mb);
+}
+
+bool aligned16(const void* ptr, int cstride, int coff) {
+  return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cstride % 8 == 0 && coff % 8 == 0;
+}
+
+}  // namespace
+
+int pp_conv_gemm_eligible(const PPConvParams& p) {
+  if (p.kh != 1 || p.kw != 1 || p.sh != 1 || p.sw != 1 || p.ph != 0 || p.pw != 0 || p.pad_replicate) return 0;
+  if (p.groups != 1 || p.split || p.epi != PP_EPI_STD || p.out_fp32 || p.M_total < 128) return 0;
+  // the segment rules of the halo kernel's flat mode: 64-channel chunks never straddle two segments
+  for (int i = 0; i < p.nseg; ++i) {
+    if (p.seg[i].cbegin % 64 != 0) return 0;
+    if (p.seg[i].cend % 64 != 0 && i != p.nseg - 1) return 0;
+  }
+  // TMA stores (and residual loads): 16-byte aligned rows
+  if (!aligned16(p.out, p.out_cstride, p.out_coff)) return 0;
+  if (p.aux0 != nullptr && !aligned16(p.aux0, p.aux0_cstride, p.aux0_coff)) return 0;
+  if (p.bias != nullptr && (reinterpret_cast<uintptr_t>(p.bias) & 7) != 0) return 0;
+  // launches of less than one wave keep the halo kernel, which narrows its tiles to fill the SMs
+  const int num_sms = gemm_num_sms();
+  if (num_sms == 0 || gemm_tiles(p, gemm_mb(p)) < num_sms) return 0;
+  return pp_conv_halo_eligible(p);   // its environment switch and tensor-map support
+}
+
+int pp_launch_conv_gemm(const PPConvParams& pin, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    attr_set = true;
+  }
+  GemmParams h;
+  memset(&h, 0, sizeof(h));
+  h.c = pin;
+  const PPConvParams& p = h.c;
+  const int mb = gemm_mb(p);
+  h.m_tiles = (int)pp_ceil_div64(p.M_total, 128 * mb);
+  h.n_tiles = pp_ceil_div(p.Cout_g_pad, 256 / mb);
+  h.chunks = pp_ceil_div(p.Cin, 64);
+  PP_REQUIRE((long long)h.m_tiles * h.n_tiles < (1LL << 31), "conv_gemm: too many tiles");
+  { const char* e = getenv("PP_CONV_NOEPI"); h.debug = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
+  PP_TRY(pp_conv_input_tmaps(p, 128 * mb, 1, true, h.tmap_a));
+  PP_TRY(pp_tmap_2d_f16(&h.tmap_out, static_cast<const __half*>(p.out) + p.out_coff, p.Cout_g, p.M_total, p.out_cstride, 64 * mb));
+  if (p.aux0 != nullptr)
+    PP_TRY(pp_tmap_2d_f16(&h.tmap_res, p.aux0 + p.aux0_coff, p.Cout_g, p.M_total, p.aux0_cstride, 64 * mb));
+  const int grid = min(h.m_tiles * h.n_tiles, gemm_num_sms());
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = SMEM_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL: see griddepcontrol.wait in the kernel
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, mb == 2 ? conv_gemm_kernel<2> : conv_gemm_kernel<1>, h));
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}

@@ -37,8 +37,8 @@ constexpr int NUM_THREADS = 384;   // warpgroup 2: warps 8-9 producers, 10-11 id
 constexpr int NUM_EPI_THREADS = 256;   // the two consumer warpgroups
 constexpr int WARP_A = 8, WARP_B = 9;
 constexpr int MAX_SA = 4, MAX_SB = 8;
-// stages and the TMA-store staging tile; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the
-// barrier block come on top (see HaloSmem)
+// stages; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the barrier block come on top (see
+// HaloSmem)
 constexpr int SMEM_BUDGET = 186 * 1024;
 
 struct HaloParams {
@@ -55,12 +55,6 @@ struct HaloParams {
   int n_img;         // images the tile index decomposes over (1 in flat mode)
   int sub_bytes;     // A-view offset between the sub-tiles: 8 pixels (spatial) or 128 pixels (flat)
   int debug;         // bit 0: skip the epilogue math/stores (PP_CONV_NOEPI=1, mainloop-only timing experiments)
-  // flat-mode layers with few K chunks are bound by the epilogue's per-thread 32-byte global stores (one L1 wavefront per
-  // lane).  tstore: the epilogue writes the fp16 tile into a 128B-swizzled shared-memory staging tile and ONE thread
-  // issues TMA stores ([128 rows x 64 columns] boxes, rows / columns beyond the tensor clipped by the TMA unit).
-  int tstore;
-  int out_stage_bytes;     // staging bytes per sub-tile: ceil(BN / 64) panels of [128 rows][128 B]
-  CUtensorMap tmap_out;
 };
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint64_t* bar) {
@@ -68,11 +62,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int 
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
       "l"(tmap), "r"(ppx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
-}
-
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(c0), "r"(c1)
-               : "memory");
 }
 
 struct TileCoord {
@@ -100,7 +89,7 @@ struct Ring {
 };
 
 // Shared-memory carve-up of both halo kernels, from the 1024-byte aligned base:
-//   SA patch stages | SB weight stages | barrier block (1 KB) | TMA-store staging (out_bytes) | 2 accumulator staging tiles
+//   SA patch stages | SB weight stages | barrier block (1 KB) | 2 accumulator staging tiles
 // The launchers call it with base == nullptr and read only `bytes`.
 struct HaloSmem {
   uint8_t* a;                  // patch stages (TMA, 128B swizzle: 1024-byte aligned)
@@ -108,15 +97,12 @@ struct HaloSmem {
   int SA, SB, a_stage_bytes, b_stage_bytes;
   uint64_t *a_full, *a_empty, *b_full, *b_empty;
   uint64_t* spare;             // one more barrier (conv_prog_kernel: layer_go)
-  uint8_t* out_stg;            // TMA-store staging tiles, 1024-byte aligned; nullptr without them
   float* acc_stg;              // ppconv::STG_BYTES per consumer warpgroup
   int bytes;                   // dynamic shared memory, including the slack that aligns the base
 };
 
-__host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage_bytes, int SB, int b_stage_bytes,
-                                              int out_bytes) {
-  const int b_off = SA * a_stage_bytes, bar_off = b_off + SB * b_stage_bytes, out_off = bar_off + 1024;
-  const int acc_off = out_off + out_bytes;
+__host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage_bytes, int SB, int b_stage_bytes) {
+  const int b_off = SA * a_stage_bytes, bar_off = b_off + SB * b_stage_bytes, acc_off = bar_off + 1024;
   HaloSmem m;
   m.SA = SA; m.SB = SB; m.a_stage_bytes = a_stage_bytes; m.b_stage_bytes = b_stage_bytes;
   m.a = base;
@@ -126,7 +112,6 @@ __host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage
   m.b_full = m.a_empty + MAX_SA;
   m.b_empty = m.b_full + MAX_SB;
   m.spare = m.b_empty + MAX_SB;
-  m.out_stg = out_bytes > 0 ? base + out_off : nullptr;   // a constant in conv_prog_kernel: one live pointer less
   m.acc_stg = reinterpret_cast<float*>(base + acc_off);
   m.bytes = 1024 + acc_off + 2 * ppconv::STG_BYTES;
   return m;
@@ -187,7 +172,7 @@ __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2],
 // (MB = h.MT m64 blocks of BN columns), then the epilogue of this warpgroup's pixel rows.  A stage is handed back to
 // its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
 // NT: see halo_tap_group.  TF32: the split-tf32 form.  PROG (conv_prog_kernel): the layer has the plain epilogue
-// (PP_EPI_STD) and no TMA-store staging tile, so neither the GRU epilogues nor the TMA-store path are compiled in.
+// (PP_EPI_STD), so the GRU epilogues are not compiled in.
 template <int BN, int MB, int NT, bool TF32 = false, bool PROG = false>
 __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
                                           int wg, int t128) {
@@ -233,15 +218,8 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
   if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
   if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
 
-  // ---- epilogue.  TMA-store path: staging tile of the sub-tile, its barrier (one warpgroup when MT == 2, both else)
+  // ---- epilogue
   const bool skip = (h.debug & 1) != 0;
-  const int bar_id = 2 + (MB == 2 ? wg : 0), bar_n = MB == 2 ? 128 : 256;
-  const bool issuer = t128 == 0 && (MB == 2 || wg == 0);
-  uint8_t* so = !PROG && h.tstore ? m.out_stg + (MB == 2 ? wg : 0) * h.out_stage_bytes : nullptr;
-  if (so != nullptr) {
-    if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
-    named_bar(bar_id, bar_n);
-  }
 #pragma unroll
   for (int b = 0; b < MB; ++b) {
     const int sub = MB == 2 ? wg : 0, rbase = MB == 2 ? 64 * b : 64 * wg;
@@ -258,27 +236,8 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
         mrow = ((long long)t.img * p.OH + oy) * p.OW + ox;
       }
       if (!mvalid || skip || cc >= bnt || n0 + cc >= p.Cout_g) return;
-      if (!TF32 && so != nullptr) {     // the TMA-store path is fp16 only (HaloParams::tstore)
-        // 16 columns = two 16-byte units of panel cc/64, row r, 128B swizzle (unit index XOR row & 7)
-        auto slot = [&](int u) {
-          const int unit = ((cc & 63) >> 3) + u;
-          return reinterpret_cast<uint4*>(so + (cc >> 6) * 16384 + r * 128 + ((unit ^ (r & 7)) << 4));
-        };
-        ppconv::epilogue_from_stage(p, src, mrow, t.g, n0 + cc, slot(0), slot(1));
-      } else {
-        ppconv::epilogue_from_stage<TF32, PROG ? PP_EPI_STD : -1>(p, src, mrow, t.g, n0 + cc, nullptr, nullptr);
-      }
+      ppconv::epilogue_from_stage<TF32, PROG ? PP_EPI_STD : -1>(p, src, mrow, t.g, n0 + cc);
     });
-  }
-  if (so != nullptr) {
-    fence_proxy_async();                                  // generic-proxy smem writes -> visible to the TMA store
-    named_bar(bar_id, bar_n);
-    if (issuer && !skip) {
-      const int row0 = (int)(((long long)t.tx * h.MT + (MB == 2 ? wg : 0)) * 128);
-      for (int pnl = 0; pnl * 64 < bnt; ++pnl)
-        tma_store_2d(&h.tmap_out, smem_u32(so + pnl * 16384), n0 + pnl * 64, row0);
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    }
   }
 }
 
@@ -353,8 +312,7 @@ __device__ __forceinline__ void halo_produce_weights(const HaloParams& h, const 
 template <bool TF32>
 __device__ __forceinline__ void halo_body(const HaloParams& h) {
   using namespace ppx;
-  const HaloSmem m =
-      halo_smem(halo_smem_base(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, h.tstore ? h.MT * h.out_stage_bytes : 0);
+  const HaloSmem m = halo_smem(halo_smem_base(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes);
   const int tid = threadIdx.x, warp = tid >> 5;
   if (tid == 0) halo_smem_init_barriers(m);
   __syncthreads();
@@ -376,7 +334,6 @@ __device__ __forceinline__ void halo_body(const HaloParams& h) {
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
         halo_tile<BN, decltype(mb)::value, halo_max_tps(BN), TF32>(h, tile, m, ra, rb, stg, wg, t128);
     });
-    if (h.tstore) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // outstanding stores of this thread complete
   } else if (warp == WARP_A) {
     if (elect_one()) {
       Ring r = {0, 0};
@@ -463,7 +420,7 @@ __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_constant__ ProgParams P) {
   using namespace ppx;
-  const HaloSmem m = halo_smem(halo_smem_base(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes, 0);
+  const HaloSmem m = halo_smem(halo_smem_base(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes);
   uint64_t* layer_go = m.spare;   // the CTA's one poller (TMA producer thread) -> consumers: layer li may start
 
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -699,71 +656,62 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloParams::tps
   h.tps = min(halo_max_tps(bn), p.kh * p.kw);
   h.b_stage_bytes = h.tps * bn * 128;
-  // TMA-store epilogue (see HaloParams::tstore): flat layers with few K chunks, plain fp16 output
-  h.tstore = 0;
-  h.out_stage_bytes = 0;
-  if (!one_wave && flat && !p.split && p.epi == PP_EPI_STD && !p.out_fp32 && p.groups == 1 && p.out_gstep == 0 && bn % 64 == 0 &&
-      p.vec_ok && h.chunks <= 16 && p.out_cstride % 8 == 0 && p.out_coff % 8 == 0 &&
-      (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
-    h.tstore = 1;
-    h.out_stage_bytes = (bn / 64) * 16384;
-  }
   int sa = 0, sb = 0;
-  if (h.tstore && !halo_stages(SMEM_BUDGET - mt * h.out_stage_bytes, h.a_stage_bytes, h.b_stage_bytes, sa, sb)) {
-    h.tstore = 0;                                 // no room for the staging tile: plain epilogue
-    h.out_stage_bytes = 0;
-  }
-  const int budget = SMEM_BUDGET - mt * h.out_stage_bytes;
-  PP_REQUIRE(halo_stages(budget, h.a_stage_bytes, h.b_stage_bytes, sa, sb), "conv_halo: patch %dx%d does not fit shared memory",
-             h.BW, h.BH);
-  if (sa == 3 && sb == MAX_SB && (budget - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
+  PP_REQUIRE(halo_stages(SMEM_BUDGET, h.a_stage_bytes, h.b_stage_bytes, sa, sb),
+             "conv_halo: patch %dx%d does not fit shared memory", h.BW, h.BH);
+  if (sa == 3 && sb == MAX_SB && (SMEM_BUDGET - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
   h.SA = sa; h.SB = sb;
-  if (h.tstore) {
-    cuuint64_t dims[2] = {(cuuint64_t)p.Cout_g, (cuuint64_t)p.M_total};
-    cuuint64_t strides[1] = {(cuuint64_t)p.out_cstride * 2};
-    cuuint32_t box[2] = {64, 128};
-    cuuint32_t es[2] = {1, 1};
-    EncodeTiledFn enc_o = encode_fn();
-    PP_REQUIRE(enc_o != nullptr, "conv_halo: cuTensorMapEncodeTiled is not available");
-    const CUresult r = enc_o(&h.tmap_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, reinterpret_cast<__half*>(p.out) + p.out_coff, dims,
-                             strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PP_REQUIRE(r == CUDA_SUCCESS, "conv_halo: cuTensorMapEncodeTiled (output) failed (%d)", (int)r);
-  }
   { const char* e = getenv("PP_CONV_NOEPI"); h.debug = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
   const long long total_tiles = count(mt, bn);
   PP_REQUIRE(total_tiles < (1LL << 31), "conv_halo: too many tiles");
+  return pp_conv_input_tmaps(p, h.BW, h.BH, flat, h.tmap);
+}
 
+}  // namespace
+
+int pp_conv_input_tmaps(const PPConvParams& p, int bw, int bh, bool flat, CUtensorMap* maps) {
   EncodeTiledFn enc = encode_fn();
-  PP_REQUIRE(enc != nullptr, "conv_halo: cuTensorMapEncodeTiled is not available");
+  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
   for (int i = 0; i < p.nseg; ++i) {
     const PPConvSeg& s = p.seg[i];
     const cuuint64_t cacc = (cuuint64_t)(p.groups - 1) * s.gstep + (s.cvalid > 0 ? s.cvalid : s.cend - s.cbegin);
     cuuint64_t dims[4] = {cacc, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
     cuuint64_t strides[3] = {(cuuint64_t)s.cstride * 2, (cuuint64_t)p.W * s.cstride * 2, (cuuint64_t)p.H * p.W * s.cstride * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)h.BW, (cuuint32_t)h.BH, 1};
+    cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1};
     if (flat) {   // pixels as one flat dimension; the last tile's tail is out of bounds -> zero-filled
       dims[1] = (cuuint64_t)p.M_total; dims[2] = 1; dims[3] = 1;
       strides[1] = strides[2] = (cuuint64_t)p.M_total * s.cstride * 2;
     }
     cuuint32_t es[4] = {1, 1, 1, 1};
-    const CUresult r = enc(&h.tmap[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(s.ptr + s.coff), dims, strides, box,
+    const CUresult r = enc(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(s.ptr + s.coff), dims, strides, box,
                            es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PP_REQUIRE(r == CUDA_SUCCESS, "conv_halo: cuTensorMapEncodeTiled failed (%d) for segment %d (cstride=%d W=%d H=%d N=%d)",
+    PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled failed (%d) for segment %d (cstride=%d W=%d H=%d N=%d)",
                (int)r, i, s.cstride, p.W, p.H, p.N);
   }
   return PP_OK;
 }
 
-}  // namespace
+int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long rows, int ld, int box_rows) {
+  EncodeTiledFn enc = encode_fn();
+  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  cuuint32_t es[2] = {1, 1};
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(base), dims, strides, box, es,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled (2-D, %d x %lld, ld %d) failed (%d)", cols, rows, ld, (int)r);
+  return PP_OK;
+}
 
 int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   HaloParams h;
   PP_TRY(halo_configure(pin, h, false));
   int num_sms = 0;
   PP_TRY(halo_num_sms(&num_sms));
-  const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, h.tstore ? h.MT * h.out_stage_bytes : 0).bytes;
+  const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes;
   return halo_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms), smem, stream);
 }
 
@@ -802,7 +750,7 @@ int pp_prog_record_conv(const PPConvParams& p) {
   const int li = r->prog.n_layers;
   PP_TRY(halo_configure(p, r->prog.layer[li], true));
   const HaloParams& h = r->prog.layer[li];
-  PP_REQUIRE(h.MT == 1 && !h.tstore && (h.c.BN == PROG_WIDTHS[0] || h.c.BN == PROG_WIDTHS[1] || h.c.BN == PROG_WIDTHS[2]),
+  PP_REQUIRE(h.MT == 1 && (h.c.BN == PROG_WIDTHS[0] || h.c.BN == PROG_WIDTHS[1] || h.c.BN == PROG_WIDTHS[2]),
              "conv program: layer tile %d x %d columns is not instantiated", h.MT, h.c.BN);
   r->prog.kind[li] = PROG_CONV;
   r->prog.n_layers++;
@@ -854,7 +802,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
   P.ts = (ts_mode && ts_printed < ts_mode) ? ts_dev : nullptr;
   const int grid = num_sms;
   *arrivals += (unsigned int)(P.n_layers * grid);
-  PP_TRY(halo_launch(conv_prog_kernel, P, grid, halo_smem(nullptr, sa, a_max, sb, b_max, 0).bytes, stream));
+  PP_TRY(halo_launch(conv_prog_kernel, P, grid, halo_smem(nullptr, sa, a_max, sb, b_max).bytes, stream));
   if (P.ts != nullptr) {      // debug: per-layer wall time of CTA 0 (serialises the stream)
     unsigned long long h[2 * PROG_MAX_LAYERS];
     PP_CUDA_CHECK(cudaStreamSynchronize(stream));

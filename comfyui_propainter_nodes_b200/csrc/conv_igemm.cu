@@ -68,7 +68,7 @@ __device__ __forceinline__ void igemm_consume(const PPConvParams& p, uint8_t* sm
     ppconv::drain_acc<BN>(acc, stg, t128, 4 + wg, [&](const float* src, int r, int c) {
       const int m = m0 + wg * 64 + r;
       if (m < p.M_total && n0 + c < p.Cout_g)
-        ppconv::epilogue_from_stage<TF32>(p, src, m, g, n0 + c, nullptr, nullptr);
+        ppconv::epilogue_from_stage<TF32>(p, src, m, g, n0 + c);
     });
   }
 }
@@ -258,6 +258,7 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
     g_last_kind = 'p';
     return pp_prog_record_conv(p);
   }
+  if (pp_conv_gemm_eligible(p)) { g_last_kind = 'g'; return pp_launch_conv_gemm(p, stream); }
   if (pp_conv_halo_eligible(p)) { g_last_kind = 'h'; return pp_launch_conv_halo(p, stream); }
   g_last_kind = 'i';
   for (int i = 0; i < p.nseg; ++i)

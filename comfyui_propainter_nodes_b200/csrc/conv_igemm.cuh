@@ -14,6 +14,8 @@
 // producers only move bytes: segment fields, Cin and the weight image are given in 2-byte units (a 128-byte K-chunk row
 // holds 32 fp32 values instead of 64 fp16), and only the MMA instruction and the epilogue differ.
 #pragma once
+#include <cuda.h>
+
 #include "pp_common.cuh"
 
 enum PPAct : int { PP_ACT_NONE = 0, PP_ACT_RELU = 1, PP_ACT_LRELU = 2, PP_ACT_SIGMOID = 3, PP_ACT_TANH = 4,
@@ -67,13 +69,21 @@ struct PPConvParams {
 };
 
 int pp_launch_conv(const PPConvParams& p, cudaStream_t stream);
-// which kernel the last pp_launch_conv of this thread went to: 'h' TMA halo-tile kernel, 'i' cp.async implicit GEMM,
-// 'p' recorded into a multi-layer program (profiling labels)
+// which kernel the last pp_launch_conv of this thread went to: 'g' flat GEMM kernel, 'h' TMA halo-tile kernel,
+// 'i' cp.async implicit GEMM, 'p' recorded into a multi-layer program (profiling labels)
 char pp_last_conv_kind();
 // conv_halo.cu: TMA halo-tile kernel for stride-1 convolutions (dispatched from pp_launch_conv when eligible;
 // PP_CONV_HALO=0 in the environment disables it).  `p` must already carry num_kc / vec_ok.
 int pp_conv_halo_eligible(const PPConvParams& p);
 int pp_launch_conv_halo(const PPConvParams& p, cudaStream_t stream);
+// conv_gemm.cu: wide-tile GEMM kernel for 1x1 convolutions and linear layers with the plain fp16 epilogue (dispatched
+// from pp_launch_conv ahead of the halo kernel when eligible).  `p` must already carry num_kc / M_total / vec_ok.
+int pp_conv_gemm_eligible(const PPConvParams& p);
+int pp_launch_conv_gemm(const PPConvParams& p, cudaStream_t stream);
+// conv_halo.cu: TMA tensor maps (fp16, 128B swizzle) of the input segments, boxes of 64 channels x bw x bh pixels;
+// flat: the N*H*W pixels as one dimension.  And a 2-D [rows][cols] map with row stride `ld` and 64 x box_rows boxes.
+int pp_conv_input_tmaps(const PPConvParams& p, int bw, int bh, bool flat, CUtensorMap* maps);
+int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long rows, int ld, int box_rows);
 
 // Multi-layer programs (conv_halo.cu): between pp_prog_begin() and pp_prog_end() every eligible convolution handed to
 // pp_launch_conv and every pp_k_dcn_sample call of this thread is RECORDED instead of launched; pp_prog_end launches

@@ -166,6 +166,9 @@ int PPConvCall::run(cudaStream_t st) {
   PPProfScope ps(*eng, "conv:" + name, rows, 2.0 * rows * macs, 0.0, st);
   const int rc = pp_launch_conv(p, st);
   if (eng->profile && !eng->prof.empty())      // label the record with the kernel the launch was dispatched to
-    eng->prof.back().name = std::string(pp_last_conv_kind() == 'h' ? "conv:halo:" : "conv:igemm:") + name;
+    eng->prof.back().name = std::string(pp_last_conv_kind() == 'g'   ? "conv:gemm:"
+                                        : pp_last_conv_kind() == 'h' ? "conv:halo:"
+                                                                     : "conv:igemm:") +
+                            name;
   return rc;
 }

@@ -1,4 +1,8 @@
-"""Micro-benchmark of the wgmma implicit-GEMM conv on representative layers (CUDA events, L2 flushed)."""
+"""Micro-benchmark of the wgmma conv kernels on representative layers (CUDA events, L2 flushed).
+
+1x1 layers (linear layers and 1x1 convolutions) also report torch.nn.functional.linear (cuBLAS, fp16 with bias) on
+the same shape in the same process, as a yardstick for the flat GEMM kernel.  PP_CONV_NOEPI=1 in the environment skips
+the epilogue math and stores of the conv kernels (main-loop timing; the outputs are then garbage)."""
 import math
 import sys
 import os
@@ -20,6 +24,13 @@ CASES = {
     "tf.fc1 (512->1960)": (1, 1, 29160, 512, 1960, 1, 1, 1, 1),
     "tf.qkv full (512->1536, M=445k)": (275, 30, 54, 512, 1536, 1, 1, 1, 1),
     "tf.proj full (512->512, M=445k)": (275, 30, 54, 512, 512, 1, 1, 1, 1),
+    # flat layers at the shapes of one bench step (80 frames at 640x360)
+    "tf.fc1 full (512->1960, M=445k)": (275, 30, 54, 512, 1960, 1, 1, 1, 1),
+    "gen.sc.embedding (512->6272, M=275k)": (102, 45, 60, 512, 6272, 1, 1, 1, 1),
+    "raft.convc1 full (1x1, 328->256, M=569k)": (158, 45, 80, 328, 256, 1, 1, 1, 1),
+    "raft.convf1 (1x1, 128->128, M=569k)": (158, 45, 80, 128, 128, 1, 1, 1, 1),
+    "gen.fp.dcn (1x1, 1152->128, M=288k)": (20, 90, 160, 1152, 128, 1, 1, 1, 1),
+    "raft.mask2 (1x1, 256->576, M=569k)": (158, 45, 80, 256, 576, 1, 1, 1, 1),
     "raft.update.conv (3x3, 256->126)": (79, 45, 80, 256, 126, 3, 3, 1, 1),
     "raft.gru.q (1x5, 384->128)": (79, 45, 80, 384, 128, 1, 5, 1, 1),
     "raft.convf2 (3x3, 128->64)": (79, 45, 80, 128, 64, 3, 3, 1, 1),
@@ -32,36 +43,51 @@ CASES = {
 }
 
 
+def _time_ms(fn, flush, reps=5):
+    """Median of `reps` single launches, each after an L2 flush (CUDA events around the call)."""
+    for _ in range(3):
+        fn()
+    ts = []
+    for _ in range(reps):
+        flush.fill_(0)
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        torch.cuda.synchronize()
+        ts.append(a.elapsed_time(b))
+    return sorted(ts)[len(ts) // 2]
+
+
 def main():
     only = sys.argv[1:]
     eng = E.Engine("cuda:0", workspace_gb=2.0)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda:0")
+    print(f"# {torch.cuda.get_device_name(0)}, PP_CONV_NOEPI={os.environ.get('PP_CONV_NOEPI', '0')}", flush=True)
     for name, (N, H, W, cin, cout, kh, kw, s, g) in CASES.items():
         if only and not any(o in name for o in only):
             continue
         w = torch.randn(cout, cin // g, kh, kw) / math.sqrt(cin * kh * kw)
-        eng.register_conv("b", w, torch.zeros(cout), g)
+        bias = torch.randn(cout) * 0.1
+        eng.register_conv("b", w, bias, g)
         x = torch.randn(N, H, W, cin, device="cuda:0", dtype=torch.float16)
         if kh != kw:
             x = torch.nn.functional.pad(x, (0, 0, kw // 2, kw // 2, kh // 2, kh // 2)).contiguous()
             pad = 0
         else:
             pad = kh // 2
-        for _ in range(3):
-            y = eng.op_conv("b", x, s, pad)
-        ts = []
-        for _ in range(5):
-            flush.fill_(0)
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            y = eng.op_conv("b", x, s, pad)
-            b.record()
-            torch.cuda.synchronize()
-            ts.append(a.elapsed_time(b))
-        ms = sorted(ts)[len(ts) // 2]
+        y = eng.op_conv("b", x, s, pad)
+        ms = _time_ms(lambda: eng.op_conv("b", x, s, pad), flush)
         M = y.shape[0] * y.shape[1] * y.shape[2]
         fl = 2.0 * M * cout * (cin // g) * kh * kw
-        print(f"{name:42s} M={M:8d} bn={eng.conv_meta['b']['bn']:3d} {ms:8.3f} ms {fl / ms / 1e9:8.1f} TFLOP/s", flush=True)
+        line = f"{name:42s} M={M:8d} bn={eng.conv_meta['b']['bn']:3d} {ms:8.3f} ms {fl / ms / 1e9:8.1f} TFLOP/s"
+        if kh == 1 and kw == 1 and g == 1:
+            x2, w2, b2 = x.reshape(-1, cin), w.reshape(cout, cin).half().cuda(), bias.half().cuda()
+            ms_cublas = _time_ms(lambda: torch.nn.functional.linear(x2, w2, b2), flush)
+            line += f" | cuBLAS {ms_cublas:8.3f} ms {fl / ms_cublas / 1e9:8.1f} TFLOP/s"
+            del x2, w2, b2
+        print(line, flush=True)
+        del x, y
 
 
 if __name__ == "__main__":
