@@ -64,53 +64,12 @@ __device__ __forceinline__ void store16(__half* dst, int nvalid, bool vec, const
   }
 }
 
-__device__ __forceinline__ void unpack16(const uint4& a, const uint4& b, float (&r)[16]) {
-  const __half2* ha = reinterpret_cast<const __half2*>(&a);
-  const __half2* hb = reinterpret_cast<const __half2*>(&b);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 fa = __half22float2(ha[i]), fb = __half22float2(hb[i]);
-    r[2 * i] = fa.x; r[2 * i + 1] = fa.y; r[8 + 2 * i] = fb.x; r[8 + 2 * i + 1] = fb.y;
-  }
-}
-
-// Epilogue operands that do not depend on the accumulator (residual / GRU h and z), fetched before the accumulator of the same
-// 16 columns is read back so the two latencies overlap instead of adding up.
-struct EpiAux {
-  uint4 a0[2], a1[2];
-  bool have;
-};
-__device__ __forceinline__ void conv_epilogue_prefetch16(const PPConvParams& p, long long mrow, int ng0, int epi, bool vec,
-                                                         EpiAux& x) {
-  x.have = false;
-  if (!vec || p.Cout_g - ng0 < 16) return;
-  const __half* s0 = nullptr;
-  const __half* s1 = nullptr;
-  if (epi == PP_EPI_STD) {
-    if (p.aux0 != nullptr) s0 = p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0;
-  } else if (epi == PP_EPI_GRU_ZR) {
-    const int half_c = p.Cout_g >> 1;
-    if (ng0 >= half_c) s0 = p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + (ng0 - half_c);
-  } else {
-    s0 = p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0;
-    s1 = p.aux1 + mrow * p.aux1_cstride + p.aux1_coff + ng0;
-  }
-  if (s0 == nullptr) return;
-  x.have = true;
-  x.a0[0] = reinterpret_cast<const uint4*>(s0)[0];
-  x.a0[1] = reinterpret_cast<const uint4*>(s0)[1];
-  if (s1 != nullptr) {
-    x.a1[0] = reinterpret_cast<const uint4*>(s1)[0];
-    x.a1[1] = reinterpret_cast<const uint4*>(s1)[1];
-  }
-}
-
 // `raw`: 16 fp32 accumulators (tile columns ng0-n0 .. +15) of output pixel `mrow` (flattened N*OH*OW index),
 // group g, first channel ng0 (within the group; ng0 < Cout_g).  `epi`/`vec` are launch-uniform.
 // The PP_EPI_STD branch's operation order is repeated per value by conv_gemm.cu's fragment epilogue (gemm_epi4); keep
 // the two in step, the flat layers' results do not depend on which kernel ran them.
 __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uint32_t (&raw)[16], long long mrow, int g,
-                                                int ng0, int epi, bool vec, const EpiAux* pre = nullptr) {
+                                                int ng0, int epi, bool vec) {
     const int nvalid = min(16, p.Cout_g - ng0);
     float v[16];
 #pragma unroll
@@ -137,8 +96,7 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
       }
       if (p.aux0 != nullptr) {
         float r[16];
-        if (pre != nullptr && pre->have) unpack16(pre->a0[0], pre->a0[1], r);
-        else load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, nvalid, vec, r);
+        load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, nvalid, vec, r);
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] += r[i];
       }
@@ -166,21 +124,15 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
       } else {
         const int c = ng0 - half_c;
         float h[16];
-        if (pre != nullptr && pre->have) unpack16(pre->a0[0], pre->a0[1], h);
-        else load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + c, nvalid, vec, h);
+        load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + c, nvalid, vec, h);
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] *= h[i];
         store16(p.out2 + mrow * p.out2_cstride + p.out2_coff + c, nvalid, vec, v);
       }
     } else {  // PP_EPI_GRU_H
       float h[16], z[16];
-      if (pre != nullptr && pre->have) {
-        unpack16(pre->a0[0], pre->a0[1], h);
-        unpack16(pre->a1[0], pre->a1[1], z);
-      } else {
-        load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, nvalid, vec, h);
-        load16(p.aux1 + mrow * p.aux1_cstride + p.aux1_coff + ng0, nvalid, vec, z);
-      }
+      load16(p.aux0 + mrow * p.aux0_cstride + p.aux0_coff + ng0, nvalid, vec, h);
+      load16(p.aux1 + mrow * p.aux1_cstride + p.aux1_coff + ng0, nvalid, vec, z);
       act16_t<PP_ACT_TANH>(v, 0.f);
 #pragma unroll
       for (int i = 0; i < 16; ++i) v[i] = (1.f - z[i]) * h[i] + z[i] * v[i];
@@ -189,12 +141,6 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
 }
 
 // ---- split-tf32 form (PPConvParams::split): fp32 [hi | lo] operands, see conv_igemm.cuh
-// hi = x rounded to tf32 (10 explicit mantissa bits, nearest, ties away), lo = x - hi (exact in fp32)
-__device__ __forceinline__ float tf32_rna(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
 // 16 consecutive channels x = hi + lo of a split tensor (hi at src, lo `lo` floats further)
 __device__ __forceinline__ void load16_split(const float* src, int lo, int nvalid, bool vec, float (&r)[16]) {
   if (vec && nvalid == 16) {
@@ -211,7 +157,7 @@ __device__ __forceinline__ void load16_split(const float* src, int lo, int nvali
 __device__ __forceinline__ void store16_split(float* dst, int lo, int nvalid, bool vec, const float (&v)[16]) {
   float h[16], l[16];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) { h[i] = tf32_rna(v[i]); l[i] = v[i] - h[i]; }
+  for (int i = 0; i < 16; ++i) { h[i] = ppx::tf32_rna(v[i]); l[i] = v[i] - h[i]; }
   if (vec && nvalid == 16) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -348,7 +294,7 @@ __device__ __forceinline__ void epilogue_from_stage(const PPConvParams& p, const
       raw[i] = __float_as_uint(v.x); raw[i + 1] = __float_as_uint(v.y);
       raw[i + 2] = __float_as_uint(v.z); raw[i + 3] = __float_as_uint(v.w);
     }
-    conv_epilogue16(p, raw, mrow, g, ng0, EPI >= 0 ? EPI : p.epi, p.vec_ok != 0, nullptr);
+    conv_epilogue16(p, raw, mrow, g, ng0, EPI >= 0 ? EPI : p.epi, p.vec_ok != 0);
   }
 }
 

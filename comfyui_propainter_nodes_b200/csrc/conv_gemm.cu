@@ -20,7 +20,6 @@
 //     ordered N-fastest: the CTAs in flight share their A rows in L2.
 // Warp roles (384 threads, one persistent CTA per SM): warpgroups 0-1 consumers, warp 8 producer (one elected thread
 // issues both loads of a stage), warps 9-11 idle (setmaxnreg works per warpgroup).
-#include <stdlib.h>
 #include <string.h>
 
 #include "conv_epilogue.cuh"
@@ -46,23 +45,6 @@ struct GemmParams {
   int debug;              // bit 0: skip the epilogue math/stores (PP_CONV_NOEPI=1, mainloop-only timing experiments)
 };
 
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, 0, 0}], [%2];" ::"r"(dst),
-      "l"(tmap), "r"(ppx::smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(tmap), "r"(ppx::smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-
 struct Smem {
   uint8_t* stages;
   uint8_t* out;
@@ -70,9 +52,7 @@ struct Smem {
   float* bias;                    // [2][256]
 };
 __device__ __forceinline__ Smem gemm_smem() {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = ppx::smem_u32(smem_raw);
-  uint8_t* base = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* base = ppx::dyn_smem_1024();
   Smem m;
   m.stages = base;
   m.out = base + STAGES * STAGE_BYTES;
@@ -196,7 +176,7 @@ __device__ __forceinline__ void gemm_tile(const GemmParams& h, const Smem& m, in
     }
     if (c0 < BN) *reinterpret_cast<float2*>(bs + c0) = bv;
   }
-  if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous tile's stores have read it
+  if (issuer) tma_store_wait_read<0>();   // the previous tile's stores have read it
   named_bar(bar_id, 128);
   const bool has_res = p.aux0 != nullptr;
   if (has_res) {
@@ -219,7 +199,7 @@ __device__ __forceinline__ void gemm_tile(const GemmParams& h, const Smem& m, in
   named_bar(bar_id, 128);
   if (issuer) {
     for (int pnl = 0; pnl < npanel; ++pnl) tma_store_2d(&h.tmap_out, smem_u32(so + pnl * PANEL), n0 + pnl * 64, row0);
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    tma_store_commit();
   }
 }
 
@@ -250,7 +230,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
     int s = 0;
     uint32_t ph = 0, rph = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) gemm_tile<MB, BN>(h, m, tile, s, ph, rph, wg, t128);
-    if (t128 == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // this warpgroup's stores complete
+    if (t128 == 0) tma_store_wait<0>();   // this warpgroup's stores complete
   } else if (warp == WARP_PRODUCER) {
     if (elect_one()) {
       int s = 0;
@@ -262,30 +242,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
         const uint32_t b_bytes = (uint32_t)(min(BN, p.Cout_g_pad - n0) * 128);
         for (int c = 0; c < h.chunks; ++c) {
           const int ci = c * 64;
-          int q = 0;
-#pragma unroll
-          for (int k = 1; k < PP_MAX_SEGS; ++k)
-            if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
+          const int q = pp_seg_of(p, ci);
           mbar_wait(&m.empty[s], ph ^ 1);
           mbar_arrive_expect_tx(&m.full[s], (uint32_t)A_BYTES + b_bytes);
           const uint32_t dst = smem_u32(m.stages + s * STAGE_BYTES);
-          tma_load_4d(dst, &h.tmap_a[q], ci - p.seg[q].cbegin, m0, &m.full[s]);
+          tma_load_4d(dst, &h.tmap_a[q], ci - p.seg[q].cbegin, m0, 0, 0, &m.full[s]);
           bulk_g2s(dst + A_BYTES, p.wpacked + ((long long)c * p.Cout_g_pad + n0) * 64, b_bytes, &m.full[s]);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
   }
-}
-
-int gemm_num_sms() {
-  static int num_sms = 0;
-  if (num_sms == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      return 0;
-  }
-  return num_sms;
 }
 
 // MB (m64 blocks per consumer warpgroup) of a layer: 256 x 128 tiles when all output channels fit one 128-wide tile
@@ -304,19 +271,15 @@ bool aligned16(const void* ptr, int cstride, int coff) {
 int pp_conv_gemm_eligible(const PPConvParams& p) {
   if (p.kh != 1 || p.kw != 1 || p.sh != 1 || p.sw != 1 || p.ph != 0 || p.pw != 0 || p.pad_replicate) return 0;
   if (p.groups != 1 || p.split || p.epi != PP_EPI_STD || p.out_fp32 || p.M_total < 128) return 0;
-  // the segment rules of the halo kernel's flat mode: 64-channel chunks never straddle two segments
-  for (int i = 0; i < p.nseg; ++i) {
-    if (p.seg[i].cbegin % 64 != 0) return 0;
-    if (p.seg[i].cend % 64 != 0 && i != p.nseg - 1) return 0;
-  }
+  if (!pp_conv_segs_chunked(p, true)) return 0;
   // TMA stores (and residual loads): 16-byte aligned rows
   if (!aligned16(p.out, p.out_cstride, p.out_coff)) return 0;
   if (p.aux0 != nullptr && !aligned16(p.aux0, p.aux0_cstride, p.aux0_coff)) return 0;
   if (p.bias != nullptr && (reinterpret_cast<uintptr_t>(p.bias) & 7) != 0) return 0;
   // launches of less than one wave keep the halo kernel, which narrows its tiles to fill the SMs
-  const int num_sms = gemm_num_sms();
-  if (num_sms == 0 || gemm_tiles(p, gemm_mb(p)) < num_sms) return 0;
-  return pp_conv_halo_eligible(p);   // its environment switch and tensor-map support
+  int num_sms = 0;
+  if (pp_num_sms(&num_sms) != PP_OK || gemm_tiles(p, gemm_mb(p)) < num_sms) return 0;
+  return pp_tmap_supported() ? 1 : 0;
 }
 
 int pp_launch_conv_gemm(const PPConvParams& pin, cudaStream_t stream) {
@@ -335,24 +298,13 @@ int pp_launch_conv_gemm(const PPConvParams& pin, cudaStream_t stream) {
   h.n_tiles = pp_ceil_div(p.Cout_g_pad, 256 / mb);
   h.chunks = pp_ceil_div(p.Cin, 64);
   PP_REQUIRE((long long)h.m_tiles * h.n_tiles < (1LL << 31), "conv_gemm: too many tiles");
-  { const char* e = getenv("PP_CONV_NOEPI"); h.debug = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
+  h.debug = pp_conv_noepi();
   PP_TRY(pp_conv_input_tmaps(p, 128 * mb, 1, true, h.tmap_a));
   PP_TRY(pp_tmap_2d_f16(&h.tmap_out, static_cast<const __half*>(p.out) + p.out_coff, p.Cout_g, p.M_total, p.out_cstride, 64 * mb));
   if (p.aux0 != nullptr)
     PP_TRY(pp_tmap_2d_f16(&h.tmap_res, p.aux0 + p.aux0_coff, p.Cout_g, p.M_total, p.aux0_cstride, 64 * mb));
-  const int grid = min(h.m_tiles * h.n_tiles, gemm_num_sms());
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL: see griddepcontrol.wait in the kernel
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, mb == 2 ? conv_gemm_kernel<2> : conv_gemm_kernel<1>, h));
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
+  int num_sms = 0;
+  PP_TRY(pp_num_sms(&num_sms));
+  return pp_conv_launch(mb == 2 ? conv_gemm_kernel<2> : conv_gemm_kernel<1>, h, min(h.m_tiles * h.n_tiles, num_sms),
+                        NUM_THREADS, SMEM_BYTES, stream);
 }

@@ -57,13 +57,6 @@ struct HaloParams {
   int debug;         // bit 0: skip the epilogue math/stores (PP_CONV_NOEPI=1, mainloop-only timing experiments)
 };
 
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
-      "l"(tmap), "r"(ppx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 struct TileCoord {
   int n_idx, tx, ty, img, g;
 };
@@ -115,13 +108,6 @@ __host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage
   m.acc_stg = reinterpret_cast<float*>(base + acc_off);
   m.bytes = 1024 + acc_off + 2 * ppconv::STG_BYTES;
   return m;
-}
-
-// The 1024-byte aligned base of the dynamic shared memory.
-__device__ __forceinline__ uint8_t* halo_smem_base() {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = ppx::smem_u32(smem_raw);
-  return smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
 }
 
 // Most filter taps whose [BN x 64] weight tiles share one 16 KB weight stage (HaloParams::tps never exceeds it).
@@ -268,10 +254,7 @@ __device__ __forceinline__ void halo_produce_patches(const HaloParams& h, const 
     const int x0 = h.flat ? t.tx * (128 * h.MT) : t.tx * (8 * h.MT) - p.pw, y0 = h.flat ? 0 : t.ty * 16 - p.ph;
     for (int c = 0; c < h.chunks; ++c) {
       const int ci = c * 64;
-      int q = 0;
-#pragma unroll
-      for (int k = 1; k < PP_MAX_SEGS; ++k)
-        if (k < p.nseg && ci >= p.seg[k].cbegin) q = k;
+      const int q = pp_seg_of(p, ci);
       const int ch0 = t.g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
       mbar_wait(&m.a_empty[r.s], r.ph ^ 1);
       mbar_arrive_expect_tx(&m.a_full[r.s], bytes);
@@ -312,7 +295,7 @@ __device__ __forceinline__ void halo_produce_weights(const HaloParams& h, const 
 template <bool TF32>
 __device__ __forceinline__ void halo_body(const HaloParams& h) {
   using namespace ppx;
-  const HaloSmem m = halo_smem(halo_smem_base(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes);
+  const HaloSmem m = halo_smem(dyn_smem_1024(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes);
   const int tid = threadIdx.x, warp = tid >> 5;
   if (tid == 0) halo_smem_init_barriers(m);
   __syncthreads();
@@ -416,11 +399,10 @@ __device__ __forceinline__ void prog_wait(const unsigned int* counter, unsigned 
     }
   }
 }
-__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_constant__ ProgParams P) {
   using namespace ppx;
-  const HaloSmem m = halo_smem(halo_smem_base(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes);
+  const HaloSmem m = halo_smem(dyn_smem_1024(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes);
   uint64_t* layer_go = m.spare;   // the CTA's one poller (TMA producer thread) -> consumers: layer li may start
 
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -513,34 +495,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    cudaDriverEntryPointQueryResult qr;
-    void* ptr = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qr) == cudaSuccess &&
-        qr == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
 }  // namespace
 
 // 0 = not eligible (caller falls back to the cp.async implicit-GEMM kernel), 1 = eligible.
 int pp_conv_halo_eligible(const PPConvParams& p) {
-  static int enabled = -1;
-  if (enabled < 0) {
-    const char* e = getenv("PP_CONV_HALO");
-    enabled = (e == nullptr || atoi(e) != 0) ? 1 : 0;
-  }
-  if (!enabled) return 0;
   if (p.sh != 1 || p.sw != 1 || p.pad_replicate) return 0;
   const bool flat = p.kh * p.kw == 1;
   if (flat) {
@@ -549,28 +507,23 @@ int pp_conv_halo_eligible(const PPConvParams& p) {
   } else if (p.Cin % 64 != 0) {
     return 0;   // packed K order is (tap, ci): 64-channel chunks must not straddle taps
   }
-  for (int i = 0; i < p.nseg; ++i) {
-    if (p.seg[i].cbegin % 64 != 0) return 0;
-    if (p.seg[i].cend % 64 != 0 && !(flat && i == p.nseg - 1)) return 0;
-  }
+  if (!pp_conv_segs_chunked(p, flat)) return 0;
   if ((p.kw - 1) * p.dw + 16 > 256 || (p.kh - 1) * p.dh + 16 > 256) return 0;
   if ((long long)p.N * p.OH * p.OW < 128) return 0;
-  return encode_fn() != nullptr ? 1 : 0;
+  return pp_tmap_supported() ? 1 : 0;
 }
 
 namespace {
 
-int halo_num_sms(int* out) {
-  static int num_sms = 0;
-  if (num_sms == 0) {
-    int dev = 0;
-    PP_CUDA_CHECK(cudaGetDevice(&dev));
-    PP_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+// The dynamic shared memory limit of the three halo kernels, raised once before the first launch.
+int halo_set_smem_limit() {
+  static bool done = false;
+  if (!done) {
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_prog_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    done = true;
   }
-  *out = num_sms;
   return PP_OK;
 }
 
@@ -587,25 +540,6 @@ bool halo_stages(int budget, int a_bytes, int b_bytes, int& sa, int& sb) {
   return false;
 }
 
-// One CTA of NUM_THREADS per SM, with programmatic dependent launch (the kernels' griddepcontrol.wait orders the data).
-template <class Params>
-int halo_launch(void (*kernel)(Params), const Params& params, int grid, int smem_bytes, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, params));
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
 // Tile shape, pipeline depth and tensor maps of one layer.  one_wave: the layer is one of a multi-layer program whose
 // layers are separated by grid-wide barriers -- prefer the least work per CTA (a second, partial wave doubles the
 // layer's latency) over fewer weight re-reads, among the tile widths the program kernel instantiates.
@@ -613,7 +547,7 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   h.c = pin;
   PPConvParams& p = h.c;
   int num_sms = 0;
-  PP_TRY(halo_num_sms(&num_sms));
+  PP_TRY(pp_num_sms(&num_sms));
   const bool flat = p.kh * p.kw == 1;
   // N tile: <= 128 columns (MT x BN accumulators of a consumer warpgroup stay within 128 registers per thread)
   const int n_tiles0 = pp_ceil_div(p.Cout_g_pad, 128);
@@ -661,7 +595,7 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
              "conv_halo: patch %dx%d does not fit shared memory", h.BW, h.BH);
   if (sa == 3 && sb == MAX_SB && (SMEM_BUDGET - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
   h.SA = sa; h.SB = sb;
-  { const char* e = getenv("PP_CONV_NOEPI"); h.debug = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
+  h.debug = pp_conv_noepi();
   const long long total_tiles = count(mt, bn);
   PP_REQUIRE(total_tiles < (1LL << 31), "conv_halo: too many tiles");
   return pp_conv_input_tmaps(p, h.BW, h.BH, flat, h.tmap);
@@ -669,50 +603,15 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
 
 }  // namespace
 
-int pp_conv_input_tmaps(const PPConvParams& p, int bw, int bh, bool flat, CUtensorMap* maps) {
-  EncodeTiledFn enc = encode_fn();
-  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
-  for (int i = 0; i < p.nseg; ++i) {
-    const PPConvSeg& s = p.seg[i];
-    const cuuint64_t cacc = (cuuint64_t)(p.groups - 1) * s.gstep + (s.cvalid > 0 ? s.cvalid : s.cend - s.cbegin);
-    cuuint64_t dims[4] = {cacc, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
-    cuuint64_t strides[3] = {(cuuint64_t)s.cstride * 2, (cuuint64_t)p.W * s.cstride * 2, (cuuint64_t)p.H * p.W * s.cstride * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-    if (flat) {   // pixels as one flat dimension; the last tile's tail is out of bounds -> zero-filled
-      dims[1] = (cuuint64_t)p.M_total; dims[2] = 1; dims[3] = 1;
-      strides[1] = strides[2] = (cuuint64_t)p.M_total * s.cstride * 2;
-    }
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    const CUresult r = enc(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(s.ptr + s.coff), dims, strides, box,
-                           es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled failed (%d) for segment %d (cstride=%d W=%d H=%d N=%d)",
-               (int)r, i, s.cstride, p.W, p.H, p.N);
-  }
-  return PP_OK;
-}
-
-int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long rows, int ld, int box_rows) {
-  EncodeTiledFn enc = encode_fn();
-  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t es[2] = {1, 1};
-  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(base), dims, strides, box, es,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled (2-D, %d x %lld, ld %d) failed (%d)", cols, rows, ld, (int)r);
-  return PP_OK;
-}
-
 int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   HaloParams h;
   PP_TRY(halo_configure(pin, h, false));
+  PP_TRY(halo_set_smem_limit());
   int num_sms = 0;
-  PP_TRY(halo_num_sms(&num_sms));
+  PP_TRY(pp_num_sms(&num_sms));
   const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes;
-  return halo_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms), smem, stream);
+  return pp_conv_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms),
+                        NUM_THREADS, smem, stream);
 }
 
 // ---- multi-layer programs ------------------------------------------------------------------------------------------
@@ -778,8 +677,9 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
   std::unique_ptr<PPProgRecorder> guard(r);
   ProgParams& P = r->prog;
   if (P.n_layers == 0) return PP_OK;
+  PP_TRY(halo_set_smem_limit());
   int num_sms = 0;
-  PP_TRY(halo_num_sms(&num_sms));
+  PP_TRY(pp_num_sms(&num_sms));
   int a_max = 1024, b_max = 2048;
   for (int i = 0; i < P.n_layers; ++i)
     if (P.kind[i] == PROG_CONV) {
@@ -802,7 +702,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
   P.ts = (ts_mode && ts_printed < ts_mode) ? ts_dev : nullptr;
   const int grid = num_sms;
   *arrivals += (unsigned int)(P.n_layers * grid);
-  PP_TRY(halo_launch(conv_prog_kernel, P, grid, halo_smem(nullptr, sa, a_max, sb, b_max).bytes, stream));
+  PP_TRY(pp_conv_launch(conv_prog_kernel, P, grid, NUM_THREADS, halo_smem(nullptr, sa, a_max, sb, b_max).bytes, stream));
   if (P.ts != nullptr) {      // debug: per-layer wall time of CTA 0 (serialises the stream)
     unsigned long long h[2 * PROG_MAX_LAYERS];
     PP_CUDA_CHECK(cudaStreamSynchronize(stream));

@@ -9,7 +9,9 @@
 // ahead through the consumers' epilogue.
 // conv_igemm_tf32_kernel is the split-tf32 form (PPConvParams::split): the same body with tf32 MMAs (k8 per 32-byte
 // k-step instead of k16) and the split epilogue.
-#include <string.h>
+// The file also holds pp_launch_conv, which picks the kernel of every convolution, and the host plumbing that the
+// halo and GEMM kernels share with this one (SM count, tensor maps).
+#include <stdlib.h>
 
 #include "conv_igemm.cuh"
 #include "conv_epilogue.cuh"
@@ -76,9 +78,7 @@ __device__ __forceinline__ void igemm_consume(const PPConvParams& p, uint8_t* sm
 template <bool TF32>
 __device__ __forceinline__ void igemm_body(const PPConvParams& p) {
   using namespace ppx;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* smem = dyn_smem_1024();
 
   const int S = p.stages;
   const int b_stage_bytes = p.BN * 128;
@@ -162,10 +162,7 @@ __device__ __forceinline__ void igemm_body(const PPConvParams& p) {
                    (uint32_t)b_stage_bytes, &full_bar[s]);
         }
         const bool kvalid = k < p.K_total;
-        int q = 0;
-#pragma unroll
-        for (int t = 1; t < PP_MAX_SEGS; ++t)
-          if (t < p.nseg && ci >= p.seg[t].cbegin) q = t;
+        const int q = pp_seg_of(p, ci);
         const __half* sbase = p.seg[q].ptr + p.seg[q].coff + g * p.seg[q].gstep + (ci - p.seg[q].cbegin);
         const long long cs = p.seg[q].cstride;
         const int dy = ky * p.dh, dx = kx * p.dw;
@@ -269,29 +266,95 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   p.stages = stages;
   const size_t smem = (size_t)stages * stage_bytes + 2 * ppconv::STG_BYTES + 1024 + 256;
-  static int num_sms = 0;
-  if (num_sms == 0) {
-    int dev = 0;
-    PP_CUDA_CHECK(cudaGetDevice(&dev));
-    PP_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+  static bool smem_limit_set = false;
+  if (!smem_limit_set) {
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_igemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    smem_limit_set = true;
   }
+  int num_sms = 0;
+  PP_TRY(pp_num_sms(&num_sms));
   const long long total_tiles = (long long)pp_ceil_div(p.M_total, BM) * (p.Cout_g_pad / p.BN) * p.groups;
   PP_REQUIRE(total_tiles < (1LL << 31), "conv: too many tiles");
   const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL: see griddepcontrol.wait in the kernel
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, p.split ? conv_igemm_tf32_kernel : conv_igemm_kernel, p));
-  PP_CUDA_CHECK(cudaGetLastError());
+  return pp_conv_launch(p.split ? conv_igemm_tf32_kernel : conv_igemm_kernel, p, grid, NUM_THREADS, smem, stream);
+}
+
+// ---- host plumbing shared with conv_halo.cu and conv_gemm.cu ----------------------------------------------------------
+int pp_num_sms(int* n) {
+  static int num_sms = 0;
+  if (num_sms == 0) {
+    int dev = 0, v = 0;
+    PP_CUDA_CHECK(cudaGetDevice(&dev));
+    PP_CUDA_CHECK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev));
+    num_sms = v;
+  }
+  *n = num_sms;
+  return PP_OK;
+}
+
+int pp_conv_noepi() {
+  const char* e = getenv("PP_CONV_NOEPI");
+  return (e != nullptr && atoi(e) != 0) ? 1 : 0;
+}
+
+namespace {
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeTiledFn encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static bool tried = false;
+  if (!tried) {
+    tried = true;
+    cudaDriverEntryPointQueryResult qr;
+    void* ptr = nullptr;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qr) == cudaSuccess &&
+        qr == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(ptr);
+  }
+  return fn;
+}
+
+}  // namespace
+
+bool pp_tmap_supported() { return encode_fn() != nullptr; }
+
+int pp_conv_input_tmaps(const PPConvParams& p, int bw, int bh, bool flat, CUtensorMap* maps) {
+  EncodeTiledFn enc = encode_fn();
+  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
+  for (int i = 0; i < p.nseg; ++i) {
+    const PPConvSeg& s = p.seg[i];
+    const cuuint64_t cacc = (cuuint64_t)(p.groups - 1) * s.gstep + (s.cvalid > 0 ? s.cvalid : s.cend - s.cbegin);
+    cuuint64_t dims[4] = {cacc, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
+    cuuint64_t strides[3] = {(cuuint64_t)s.cstride * 2, (cuuint64_t)p.W * s.cstride * 2, (cuuint64_t)p.H * p.W * s.cstride * 2};
+    cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1};
+    if (flat) {   // pixels as one flat dimension; the last tile's tail is out of bounds -> zero-filled
+      dims[1] = (cuuint64_t)p.M_total; dims[2] = 1; dims[3] = 1;
+      strides[1] = strides[2] = (cuuint64_t)p.M_total * s.cstride * 2;
+    }
+    cuuint32_t es[4] = {1, 1, 1, 1};
+    const CUresult r = enc(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(s.ptr + s.coff), dims, strides, box,
+                           es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled failed (%d) for segment %d (cstride=%d W=%d H=%d N=%d)",
+               (int)r, i, s.cstride, p.W, p.H, p.N);
+  }
+  return PP_OK;
+}
+
+int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long rows, int ld, int box_rows) {
+  EncodeTiledFn enc = encode_fn();
+  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  cuuint32_t es[2] = {1, 1};
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(base), dims, strides, box, es,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled (2-D, %d x %lld, ld %d) failed (%d)", cols, rows, ld, (int)r);
   return PP_OK;
 }

@@ -72,18 +72,66 @@ int pp_launch_conv(const PPConvParams& p, cudaStream_t stream);
 // which kernel the last pp_launch_conv of this thread went to: 'g' flat GEMM kernel, 'h' TMA halo-tile kernel,
 // 'i' cp.async implicit GEMM, 'p' recorded into a multi-layer program (profiling labels)
 char pp_last_conv_kind();
-// conv_halo.cu: TMA halo-tile kernel for stride-1 convolutions (dispatched from pp_launch_conv when eligible;
-// PP_CONV_HALO=0 in the environment disables it).  `p` must already carry num_kc / vec_ok.
+// conv_halo.cu: TMA halo-tile kernel for stride-1 convolutions (dispatched from pp_launch_conv when eligible).
+// `p` must already carry num_kc / vec_ok.
 int pp_conv_halo_eligible(const PPConvParams& p);
 int pp_launch_conv_halo(const PPConvParams& p, cudaStream_t stream);
 // conv_gemm.cu: wide-tile GEMM kernel for 1x1 convolutions and linear layers with the plain fp16 epilogue (dispatched
 // from pp_launch_conv ahead of the halo kernel when eligible).  `p` must already carry num_kc / M_total / vec_ok.
 int pp_conv_gemm_eligible(const PPConvParams& p);
 int pp_launch_conv_gemm(const PPConvParams& p, cudaStream_t stream);
-// conv_halo.cu: TMA tensor maps (fp16, 128B swizzle) of the input segments, boxes of 64 channels x bw x bh pixels;
-// flat: the N*H*W pixels as one dimension.  And a 2-D [rows][cols] map with row stride `ld` and 64 x box_rows boxes.
+
+// ---- host plumbing of the conv kernels (conv_igemm.cu, next to pp_launch_conv)
+// SM count of the current device, queried once.
+int pp_num_sms(int* n);
+// cuTensorMapEncodeTiled is available: the halo and GEMM kernels load their operands with TMA.
+bool pp_tmap_supported();
+// TMA tensor maps (fp16, 128B swizzle) of the input segments, boxes of 64 channels x bw x bh pixels; flat: the N*H*W
+// pixels as one dimension.  And a 2-D [rows][cols] map with row stride `ld` and 64 x box_rows boxes.
 int pp_conv_input_tmaps(const PPConvParams& p, int bw, int bh, bool flat, CUtensorMap* maps);
 int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long rows, int ld, int box_rows);
+// 1 when PP_CONV_NOEPI=1 is set: the halo and GEMM kernels skip the epilogue math and stores (main-loop-only timing)
+int pp_conv_noepi();
+
+// The TMA kernels load 64-channel K chunks from one segment each, so no chunk may straddle two segments: every segment
+// starts on a chunk boundary, and only the last segment of a flat (1x1) layer may end inside one (TMA zero-fills the
+// ragged channel tail).
+inline bool pp_conv_segs_chunked(const PPConvParams& p, bool flat) {
+  for (int i = 0; i < p.nseg; ++i) {
+    if (p.seg[i].cbegin % 64 != 0) return false;
+    if (p.seg[i].cend % 64 != 0 && !(flat && i == p.nseg - 1)) return false;
+  }
+  return true;
+}
+
+// The segment that holds conv-input channel `ci`.
+__device__ __forceinline__ int pp_seg_of(const PPConvParams& p, int ci) {
+  int q = 0;
+#pragma unroll
+  for (int t = 1; t < PP_MAX_SEGS; ++t)
+    if (t < p.nseg && ci >= p.seg[t].cbegin) q = t;
+  return q;
+}
+
+// A persistent conv kernel launch (1-D grid) with programmatic dependent launch: the kernel's griddepcontrol.wait
+// orders its reads after the previous kernel in the stream.
+template <class Params>
+int pp_conv_launch(void (*kernel)(Params), const Params& params, int grid, int threads, size_t smem_bytes,
+                   cudaStream_t stream) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem_bytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  PP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, params));
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
 
 // Multi-layer programs (conv_halo.cu): between pp_prog_begin() and pp_prog_end() every eligible convolution handed to
 // pp_launch_conv and every pp_k_dcn_sample call of this thread is RECORDED instead of launched; pp_prog_end launches

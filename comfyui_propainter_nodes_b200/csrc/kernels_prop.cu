@@ -533,9 +533,8 @@ int imgprop_run(const void* in4, void* bwd, void* fwd, const void* ff, const voi
                 int H, int W, int* scratch, cudaStream_t st) {
   static int grid_max = 0;      // one per storage type: the fp32 kernel has its own register footprint
   if (grid_max == 0) {
-    int dev = 0, sms = 0, per_sm = 0;
-    PP_CUDA_CHECK(cudaGetDevice(&dev));
-    PP_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int sms = 0, per_sm = 0;
+    PP_TRY(pp_num_sms(&sms));
     PP_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, imgprop_persistent<S>, 256, 0));
     PP_REQUIRE(per_sm >= 1, "imgprop: persistent kernel does not fit an SM");
     grid_max = sms * (per_sm < 2 ? per_sm : 2);

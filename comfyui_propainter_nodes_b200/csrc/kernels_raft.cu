@@ -8,12 +8,6 @@ namespace {
 
 constexpr int TPB = 256;
 
-// x rounded to tf32 (nearest, ties away): the hi half of a split pair; the lo half is x - hi (exact)
-__device__ __forceinline__ float tf32_round(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
 inline int nblocks(long long n, int per = TPB) { return (int)((n + per - 1) / per); }
 
 // ------------------------------------------------------------------------------------------------
@@ -113,12 +107,12 @@ __device__ __forceinline__ float2 ld_split2(const float* p, int C) {
   return make_float2(h.x + l.x, h.y + l.y);
 }
 __device__ __forceinline__ void st_split2(float* p, int C, float a, float b) {
-  const float ha = tf32_round(a), hb = tf32_round(b);
+  const float ha = ppx::tf32_rna(a), hb = ppx::tf32_rna(b);
   *reinterpret_cast<float2*>(p) = make_float2(ha, hb);
   *reinterpret_cast<float2*>(p + C) = make_float2(a - ha, b - hb);
 }
 __device__ __forceinline__ void st_split1(float* p, int C, float a) {
-  const float h = tf32_round(a);
+  const float h = ppx::tf32_rna(a);
   p[0] = h;
   p[C] = a - h;
 }
@@ -287,7 +281,7 @@ __global__ void __launch_bounds__(LOOKUP_WARPS * 32) corr_lookup(CorrLevels<E> l
         const float bot = t[TAP_COLS] + a * (t[TAP_COLS + 1] - t[TAP_COLS]);
         const float v = top + b * (bot - top);
         if constexpr (F32) {
-          const float hi = tf32_round(v);
+          const float hi = ppx::tf32_rna(v);
           o[l * 81 + r] = hi;
           o[out_cs + l * 81 + r] = v - hi;
         } else {

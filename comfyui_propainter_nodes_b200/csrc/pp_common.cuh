@@ -68,19 +68,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 // launch-latency-bound recurrent layers).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
-#ifdef PP_MBAR_UNBOUNDED   // A/B builds: the plain spin
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra WAIT_DONE;\n"
-      "bra WAIT_LOOP;\n"
-      "WAIT_DONE:\n"
-      "}\n" ::"r"(addr),
-      "r"(parity)
-      : "memory");
-#else
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
@@ -97,7 +84,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "}\n" ::"r"(addr),
       "r"(parity)
       : "memory");
-#endif
 }
 
 // ------------------------------------------------------------------ grid-wide barrier (persistent kernels)
@@ -142,6 +128,8 @@ __device__ __forceinline__ void cp_async_wait() {
 }
 // generic-proxy writes -> visible to the async proxy (wgmma / TMA reads of shared memory)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// the same for generic-proxy writes to global memory that a later TMA load reads
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 // Bulk async copy global -> shared through the TMA engine (SASS: UBLKCP), completion on an mbarrier.
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -149,6 +137,43 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
       "l"(src), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
+}
+
+// TMA tensor loads (global -> shared, box and swizzle given by the CUtensorMap at `tmap`), completion on an mbarrier.
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
+      "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
+      "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// TMA tensor store (shared -> global) into this thread's bulk group; tma_store_commit closes the group, and
+// tma_store_wait_read<N> / tma_store_wait<N> wait until at most N groups still read shared memory / are incomplete.
+__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void tma_store_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// The 1024-byte aligned base of the dynamic shared memory (128B-swizzled TMA / wgmma tiles need that alignment).
+// Launches reserve 1024 bytes of slack for it.
+__device__ __forceinline__ uint8_t* dyn_smem_1024() {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  return smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
 }
 
 // ------------------------------------------------------------------ wgmma (warpgroup MMA, accumulators in registers)
@@ -207,6 +232,14 @@ __device__ __forceinline__ bool elect_one() {
       "}\n"
       : "=r"(pred));
   return pred != 0;
+}
+
+// x rounded to tf32 (10 explicit mantissa bits, nearest, ties away): the hi half of a split-tf32 pair (conv_igemm.cuh);
+// the lo half x - hi is exact in fp32
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }

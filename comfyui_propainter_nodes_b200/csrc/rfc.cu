@@ -33,8 +33,7 @@ inline void shard(int n, int parts, int k, int& lo, int& hi) {   // contiguous n
 
 inline bool rfc_use_programs() {
   const char* s = getenv("PP_PROG");
-  const char* hk = getenv("PP_CONV_HALO");      // programs are made of TMA halo-kernel layers
-  return (s == nullptr || atoi(s) != 0) && (hk == nullptr || atoi(hk) != 0);
+  return s == nullptr || atoi(s) != 0;
 }
 
 // Temporal reach of the encoder: four P3D blocks, each a (3,1,1) dilation-2 conv (t-2, t, t+2) => a frame's

@@ -4,38 +4,18 @@ ptxas reports C7519 / C7520 when it has to inject `warpgroup.arrive` waits into 
 waits for the previous one), and C7512 when it serializes them for lack of registers.  Neither shows up in any output,
 only in the kernel's speed, so the compiler's own report and the SASS are checked here, together with the stack and
 spill report of both tile shapes (the 128 accumulator registers per thread must stay in registers)."""
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "comfyui_propainter_nodes_b200", "csrc")
+from tests.conv_codegen import compile_csrc, sass_functions, stack_and_spills
+
 KERNEL = "16conv_gemm_kernel"     # mangled conv_gemm_kernel<MB>(GemmParams), anonymous namespace
 
 
-def _cuda_tool(name):
-    path = shutil.which(name)
-    if path is None:
-        cand = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", name)
-        path = cand if os.path.exists(cand) else None
-    return path
-
-
 @pytest.fixture(scope="module")
-def gemm_build(tmp_path_factory):
-    nvcc = _cuda_tool("nvcc")
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    obj = str(tmp_path_factory.mktemp("gemm") / "conv_gemm.o")
-    # the library's flags (csrc/Makefile) plus the ptxas report
-    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--use_fast_math", "-Xptxas", "-v",
-           "-c", os.path.join(CSRC, "conv_gemm.cu"), "-o", obj]
-    res = subprocess.run(cmd, cwd=CSRC, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-4000:]
-    return obj, res.stdout + res.stderr
+def gemm_build():
+    return compile_csrc("conv_gemm.cu")
 
 
 def test_gemm_kernel_has_no_wgmma_serialization_warnings(gemm_build):
@@ -46,26 +26,14 @@ def test_gemm_kernel_has_no_wgmma_serialization_warnings(gemm_build):
 
 def test_gemm_kernel_has_no_stack_or_spills(gemm_build):
     _, log = gemm_build
-    lines = log.splitlines()
-    found = 0
-    for i, ln in enumerate(lines):
-        if "Function properties for" in ln and KERNEL in ln:
-            found += 1
-            props = lines[i + 1]
-            m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", props)
-            assert m is not None, props
-            assert m.groups() == ("0", "0", "0"), (ln, props)
-    assert found == 2, "expected the two tile shapes (MB = 1, 2) of conv_gemm_kernel"
+    props = stack_and_spills(log, KERNEL)
+    assert len(props) == 2, "expected the two tile shapes (MB = 1, 2) of conv_gemm_kernel"
+    assert all(p == (0, 0, 0) for p in props), props
 
 
 def test_gemm_kernel_sass_waits_once_per_commit_group(gemm_build):
-    cuobjdump = _cuda_tool("cuobjdump")
-    if cuobjdump is None:
-        pytest.skip("cuobjdump not found")
     obj, _ = gemm_build
-    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    funcs = re.split(r"\n\s*Function : ", sass)
-    bodies = [f for f in funcs if f.startswith("_Z") and KERNEL in f.split("\n", 1)[0]]
+    bodies = sass_functions(obj, KERNEL)
     assert len(bodies) == 2, "conv_gemm_kernel<1> / <2> not found in the SASS"
     for body in bodies:
         # a commit group holds 4 * MB HGMMAs (one 64-channel K chunk); a serialized sequence has a wait after each one.

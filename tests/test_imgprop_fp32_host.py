@@ -10,7 +10,7 @@ import torch
 
 from comfyui_propainter_nodes_b200 import engine as E
 from comfyui_propainter_nodes_b200 import propainter_inference as PI
-from tests.test_halo_codegen import CSRC, _cuda_tool
+from tests.conv_codegen import CSRC, _cuda_tool
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 

@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from comfyui_propainter_nodes_b200 import engine as E
-from tests.test_halo_codegen import CSRC, _cuda_tool
+from tests.conv_codegen import CSRC, _cuda_tool
 
 TF32_KERNEL = "21conv_halo_tf32_kernelENS_10HaloParamsE"    # mangled conv_halo_tf32_kernel(HaloParams)
 
