@@ -48,6 +48,36 @@ struct ArenaGuard {
   ~ArenaGuard() { if (!keep) a.release(m); }
 };
 
+// pp_op_instnorm / pp_op_corr_pyramid take tensors of either precision as void* plus an fp32 flag: E is the element type
+template <class E>
+static int op_instnorm(PPEngine& e, const void* x, const void* residual, void* out, int N, int HW, int C, int relu,
+                       cudaStream_t st) {
+  ArenaGuard guard(e.arena);
+  float* sums;
+  PP_TRY(pp_alloc(e, &sums, pp_k_instnorm_scratch_floats(N, HW, C), "instnorm sums"));
+  PP_TRY(pp_k_instnorm_stats(static_cast<const E*>(x), N, HW, C, sums, st));
+  PP_TRY(pp_k_instnorm_apply(static_cast<const E*>(x), sums, static_cast<const E*>(residual), static_cast<E*>(out), N,
+                             HW, C, relu, st));
+  PP_CUDA_CHECK(cudaStreamSynchronize(st));   // the scratch goes back to the arena on return
+  return PP_OK;
+}
+
+template <class E>
+static int op_corr_pyramid(PPEngine& e, const void* fmap1, const void* fmap2, int pairs, int h8, int w8, void* l0,
+                           void* l1, void* l2, void* l3, cudaStream_t st) {
+  ArenaGuard guard(e.arena);
+  const int P = h8 * w8, P_pad = pp_raft_corr_pad(P);
+  E* fpack;   // 256 values per row, fp32: the three segments [hi; hi; lo]
+  PP_TRY(pp_alloc(e, &fpack, (size_t)pairs * P_pad * 256 * (sizeof(E) == 4 ? 3 : 1), "fmap packed"));
+  PP_TRY(pp_k_pack_b_operand(static_cast<const E*>(fmap2), fpack, pairs, P, P_pad, 256, st));
+  e.launches++;
+  E* const corr[4] = {static_cast<E*>(l0), static_cast<E*>(l1), static_cast<E*>(l2), static_cast<E*>(l3)};
+  PP_TRY(pp_raft_corr_volume<E>(e, static_cast<const E*>(fmap1), fpack, pairs, P, P_pad, corr[0], st));
+  PP_TRY(pp_raft_corr_pool(e, corr, (long long)pairs * P, h8, w8, st));
+  PP_CUDA_CHECK(cudaStreamSynchronize(st));
+  return PP_OK;
+}
+
 extern "C" {
 
 const char* pp_version(void) { return "propainter_b200 1 sm_90a"; }
@@ -160,7 +190,7 @@ int pp_raft_bidir(pp_handle h, const float* frames, int T, int H, int W, int ite
   PP_HANDLE(h);
   PP_REQUIRE(frames && flows_f && flows_b, "pp_raft_bidir: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_raft(e, frames, T, H, W, iters, flows_f, flows_b, false, as_stream(stream));
+  return pp_stage_raft<__half>(e, frames, T, H, W, iters, flows_f, flows_b, as_stream(stream));
 }
 
 int pp_raft_bidir_fp32(pp_handle h, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
@@ -168,7 +198,7 @@ int pp_raft_bidir_fp32(pp_handle h, const float* frames, int T, int H, int W, in
   PP_HANDLE(h);
   PP_REQUIRE(frames && flows_f && flows_b, "pp_raft_bidir_fp32: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_raft(e, frames, T, H, W, iters, flows_f, flows_b, true, as_stream(stream));
+  return pp_stage_raft<float>(e, frames, T, H, W, iters, flows_f, flows_b, as_stream(stream));
 }
 
 int pp_flow_complete(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T, int H,
@@ -198,8 +228,8 @@ int pp_image_propagate(pp_handle h, const float* frames, const float* masks, con
   PP_REQUIRE(frames && masks && flows_f && flows_b && updated_frames && updated_masks,
              "pp_image_propagate: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_image_propagate(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks, false,
-                                  as_stream(stream));
+  return pp_stage_image_propagate<__half>(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks,
+                                          as_stream(stream));
 }
 
 int pp_image_propagate_fp32(pp_handle h, const float* frames, const float* masks, const float* flows_f,
@@ -209,8 +239,8 @@ int pp_image_propagate_fp32(pp_handle h, const float* frames, const float* masks
   PP_REQUIRE(frames && masks && flows_f && flows_b && updated_frames && updated_masks,
              "pp_image_propagate_fp32: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_image_propagate(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks, true,
-                                  as_stream(stream));
+  return pp_stage_image_propagate<float>(e, frames, masks, flows_f, flows_b, T, H, W, updated_frames, updated_masks,
+                                         as_stream(stream));
 }
 
 int pp_gen_begin_subset(pp_handle h, const float* updated_frames, const float* masks_dilated,
@@ -416,7 +446,7 @@ int pp_op_conv(pp_handle h, const char* name, const void* x_f16, int N, int H, i
   PPConvCall c(e, name, N, H, W);
   c.in(static_cast<const __half*>(x_f16), w->cin_g * w->groups, 0, w->cin_g, w->groups > 1 ? w->cin_g : 0)
       .geom(stride, stride, pad, pad, dil, dil, replicate)
-      .out(out_f16, w->cout_g * w->groups, 0, 0, w->groups > 1 ? w->cout_g : 0)
+      .out(static_cast<__half*>(out_f16), w->cout_g * w->groups, 0, w->groups > 1 ? w->cout_g : 0)
       .act(act, slope);
   if (residual_f16 != nullptr) c.residual(static_cast<const __half*>(residual_f16), w->cout_g * w->groups, 0);
   return c.run(as_stream(stream));
@@ -428,7 +458,7 @@ int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l
   e.launches++;
   return pp_k_corr_lookup(static_cast<const __half*>(l0), static_cast<const __half*>(l1),
                           static_cast<const __half*>(l2), static_cast<const __half*>(l3), coords,
-                          static_cast<__half*>(out_f16), 328, nq, h8 * w8, h8, w8, as_stream(stream));
+                          static_cast<__half*>(out_f16), 328, nq, h8, w8, as_stream(stream));
 }
 
 int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, int x0_co, int x0_ch, const float* x1,
@@ -439,18 +469,18 @@ int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, in
   PP_REQUIRE(name && x0 && out, "pp_op_conv_tf32: null pointer");
   PP_REQUIRE(epi == PP_EPI_STD || (aux0 && aux1), "pp_op_conv_tf32: the GRU epilogues need aux0 and aux1");
   PPConvCall c(e, name, N, H, W);
-  c.tf32().in_split(x0, x0_C, x0_co, x0_ch);
-  if (x1 != nullptr) c.in_split(x1, x1_C, x1_co, x1_ch);
+  c.in(x0, x0_C, x0_co, x0_ch);
+  if (x1 != nullptr) c.in(x1, x1_C, x1_co, x1_ch);
   c.geom(sh, sw, ph, pw);
-  if (out_fp32) c.out(out, out_C, out_co, 1);
-  else c.out_split(out, out_C, out_co);
+  if (out_fp32) c.out_f32(out, out_C, out_co);
+  else c.out(out, out_C, out_co);
   if (epi == PP_EPI_GRU_ZR) {
-    c.gru_zr_split(aux0, aux0_C, aux0_co, aux1, aux1_C, aux1_co);
+    c.gru_zr(aux0, aux0_C, aux0_co, aux1, aux1_C, aux1_co);
   } else if (epi == PP_EPI_GRU_H) {
-    c.gru_h_split(aux0, aux0_C, aux0_co, aux1, aux1_C, aux1_co);
+    c.gru_h(aux0, aux0_C, aux0_co, aux1, aux1_C, aux1_co);
   } else {
     c.act(act, slope, scale, act2);
-    if (aux0 != nullptr) c.residual_split(aux0, aux0_C, aux0_co);
+    if (aux0 != nullptr) c.residual(aux0, aux0_C, aux0_co);
   }
   return c.run(as_stream(stream));
 }
@@ -459,56 +489,30 @@ int pp_op_instnorm(pp_handle h, const void* x, const void* residual, void* out, 
                    void* stream) {
   PP_HANDLE(h);
   PP_REQUIRE(x && out, "pp_op_instnorm: null pointer");
-  ArenaGuard guard(e.arena);
-  float* sums;
-  PP_TRY(pp_alloc(e, &sums, pp_k_instnorm_scratch_floats(N, HW, C), "instnorm sums"));
-  cudaStream_t st = as_stream(stream);
-  if (fp32) {
-    PP_TRY(pp_k_instnorm_stats_f32(static_cast<const float*>(x), N, HW, C, sums, st));
-    PP_TRY(pp_k_instnorm_apply_f32(static_cast<const float*>(x), sums, static_cast<const float*>(residual),
-                                   static_cast<float*>(out), N, HW, C, relu, st));
-  } else {
-    PP_TRY(pp_k_instnorm_stats(static_cast<const __half*>(x), N, HW, C, sums, st));
-    PP_TRY(pp_k_instnorm_apply(static_cast<const __half*>(x), sums, static_cast<const __half*>(residual),
-                               static_cast<__half*>(out), N, HW, C, relu, st));
-  }
-  PP_CUDA_CHECK(cudaStreamSynchronize(st));   // the scratch goes back to the arena on return
-  return PP_OK;
+  return fp32 ? op_instnorm<float>(e, x, residual, out, N, HW, C, relu, as_stream(stream))
+              : op_instnorm<__half>(e, x, residual, out, N, HW, C, relu, as_stream(stream));
 }
 
 int pp_op_corr_pyramid(pp_handle h, const void* fmap1, const void* fmap2, int pairs, int h8, int w8, int fp32, void* l0,
                        void* l1, void* l2, void* l3, void* stream) {
   PP_HANDLE(h);
   PP_REQUIRE(fmap1 && fmap2 && l0 && l1 && l2 && l3 && pairs >= 1, "pp_op_corr_pyramid: bad argument");
-  ArenaGuard guard(e.arena);
-  cudaStream_t st = as_stream(stream);
-  const int P = h8 * w8, P_pad = pp_raft_corr_pad(P);
-  uint8_t* fpack;
-  PP_TRY(pp_alloc(e, &fpack, (size_t)pairs * P_pad * 256 * (fp32 ? 12 : 2), "fmap packed"));
-  if (fp32) PP_TRY(pp_k_pack_b_operand_split(static_cast<const float*>(fmap2), reinterpret_cast<float*>(fpack), pairs, P,
-                                             P_pad, 256, st));
-  else PP_TRY(pp_k_pack_b_operand(static_cast<const __half*>(fmap2), reinterpret_cast<__half*>(fpack), pairs, P, P_pad,
-                                  256, st));
-  e.launches++;
-  PP_TRY(pp_raft_corr_volume(e, fmap1, fpack, pairs, P, P_pad, fp32 != 0, l0, st));
-  void* const corr[4] = {l0, l1, l2, l3};
-  PP_TRY(pp_raft_corr_pool(e, corr, (long long)pairs * P, h8, w8, fp32 != 0, st));
-  PP_CUDA_CHECK(cudaStreamSynchronize(st));
-  return PP_OK;
+  return fp32 ? op_corr_pyramid<float>(e, fmap1, fmap2, pairs, h8, w8, l0, l1, l2, l3, as_stream(stream))
+              : op_corr_pyramid<__half>(e, fmap1, fmap2, pairs, h8, w8, l0, l1, l2, l3, as_stream(stream));
 }
 
 int pp_op_corr_lookup_f32(pp_handle h, const float* l0, const float* l1, const float* l2, const float* l3,
                           const float* coords, float* out, long long nq, int h8, int w8, void* stream) {
   PP_HANDLE(h);
   e.launches++;
-  return pp_k_corr_lookup_f32(l0, l1, l2, l3, coords, out, 352, nq, h8, w8, as_stream(stream));
+  return pp_k_corr_lookup(l0, l1, l2, l3, coords, out, 352, nq, h8, w8, as_stream(stream));
 }
 
 int pp_op_convex_upsample(pp_handle h, const float* coords1, const void* mask, float* out, int B, int h8, int w8, int fp32,
                           void* stream) {
   PP_HANDLE(h);
   e.launches++;
-  if (fp32) return pp_k_convex_upsample_f32(coords1, static_cast<const float*>(mask), out, B, h8, w8, as_stream(stream));
+  if (fp32) return pp_k_convex_upsample(coords1, static_cast<const float*>(mask), out, B, h8, w8, as_stream(stream));
   return pp_k_convex_upsample(coords1, static_cast<const __half*>(mask), out, B, h8, w8, as_stream(stream));
 }
 
@@ -526,7 +530,7 @@ int pp_op_imgprop_step_f32(pp_handle h, const float* cur4, const float* prop_in4
   PP_HANDLE(h);
   PP_REQUIRE(cur4 && prop_in4 && prop_out4 && flow_prop && flow_check, "pp_op_imgprop_step_f32: null pointer");
   e.launches++;
-  return pp_k_imgprop_step_f32(cur4, prop_in4, prop_out4, flow_prop, flow_check, H, W, as_stream(stream));
+  return pp_k_imgprop_step(cur4, prop_in4, prop_out4, flow_prop, flow_check, H, W, as_stream(stream));
 }
 
 int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,

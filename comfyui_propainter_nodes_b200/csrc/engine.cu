@@ -56,8 +56,13 @@ PPConvCall& PPConvCall::geom(int sh, int sw, int ph, int pw, int dh, int dw, int
   return *this;
 }
 
-PPConvCall& PPConvCall::out(void* ptr, int cs, int co, int fp32, int gstep) {
-  p.out = ptr; p.out_cstride = cs; p.out_coff = co; p.out_fp32 = fp32; p.out_gstep = gstep;
+PPConvCall& PPConvCall::out(__half* ptr, int cs, int co, int gstep) {
+  p.out = ptr; p.out_cstride = cs; p.out_coff = co; p.out_fp32 = 0; p.out_gstep = gstep;
+  return *this;
+}
+
+PPConvCall& PPConvCall::out_f32(float* ptr, int cs, int co) {
+  p.out = ptr; p.out_cstride = cs; p.out_coff = co; p.out_fp32 = 1; p.out_gstep = 0;
   return *this;
 }
 
@@ -85,40 +90,36 @@ PPConvCall& PPConvCall::gru_h(const __half* h, int h_cs, int h_co, const __half*
   return *this;
 }
 
-PPConvCall& PPConvCall::tf32() {
-  p.split = 1;
-  return *this;
-}
-
-PPConvCall& PPConvCall::in_split(const float* ptr, int C, int co, int channels) {
+PPConvCall& PPConvCall::in(const float* ptr, int C, int co, int channels) {
   if (err != PP_OK) return *this;
-  if (!p.split || n_split_in >= PP_MAX_SEGS / 3) {
-    pp_set_error("conv %s: in_split needs tf32() and at most %d inputs", name.c_str(), PP_MAX_SEGS / 3);
+  if (n_split_in >= PP_MAX_SEGS / 3) {
+    pp_set_error("conv %s: more than %d split-tf32 inputs", name.c_str(), PP_MAX_SEGS / 3);
     err = PP_ERR_ARG;
     return *this;
   }
+  p.split = 1;
   split_in[n_split_in++] = SplitIn{ptr, C, co, channels};
   return *this;
 }
 
-PPConvCall& PPConvCall::out_split(float* ptr, int C, int co) {
+PPConvCall& PPConvCall::out(float* ptr, int C, int co) {
   p.out = ptr; p.out_cstride = 2 * C; p.out_coff = co; p.out_lo = C; p.out_fp32 = 0; p.out_gstep = 0;
   return *this;
 }
 
-PPConvCall& PPConvCall::residual_split(const float* ptr, int C, int co) {
+PPConvCall& PPConvCall::residual(const float* ptr, int C, int co) {
   p.aux0 = reinterpret_cast<const __half*>(ptr); p.aux0_cstride = 2 * C; p.aux0_coff = co; p.aux0_lo = C;
   return *this;
 }
 
-PPConvCall& PPConvCall::gru_zr_split(const float* h, int h_C, int h_co, float* rh, int rh_C, int rh_co) {
+PPConvCall& PPConvCall::gru_zr(const float* h, int h_C, int h_co, float* rh, int rh_C, int rh_co) {
   p.epi = PP_EPI_GRU_ZR;
   p.aux0 = reinterpret_cast<const __half*>(h); p.aux0_cstride = 2 * h_C; p.aux0_coff = h_co; p.aux0_lo = h_C;
   p.out2 = reinterpret_cast<__half*>(rh); p.out2_cstride = 2 * rh_C; p.out2_coff = rh_co; p.out2_lo = rh_C;
   return *this;
 }
 
-PPConvCall& PPConvCall::gru_h_split(const float* h, int h_C, int h_co, const float* z, int z_C, int z_co) {
+PPConvCall& PPConvCall::gru_h(const float* h, int h_C, int h_co, const float* z, int z_C, int z_co) {
   p.epi = PP_EPI_GRU_H;
   p.aux0 = reinterpret_cast<const __half*>(h); p.aux0_cstride = 2 * h_C; p.aux0_coff = h_co; p.aux0_lo = h_C;
   p.aux1 = reinterpret_cast<const __half*>(z); p.aux1_cstride = 2 * z_C; p.aux1_coff = z_co; p.aux1_lo = z_C;
@@ -129,7 +130,7 @@ int PPConvCall::run(cudaStream_t st) {
   if (err != PP_OK) return err;
   if (p.split) {
     // (hi, lo, hi) passes over the inputs, in the kernel's 2-byte units: an fp32 channel is two of them
-    PP_REQUIRE(p.nseg == 0 && n_split_in > 0, "conv %s: split-tf32 inputs must all come from in_split", name.c_str());
+    PP_REQUIRE(p.nseg == 0 && n_split_in > 0, "conv %s: split-tf32 (float*) and fp16 inputs cannot be mixed", name.c_str());
     for (int pass = 0; pass < 3; ++pass)
       for (int i = 0; i < n_split_in; ++i) {
         const SplitIn& s = split_in[i];

@@ -49,11 +49,9 @@ struct PPEngine {
     __half* flows_f4 = nullptr;   // [T-1][h][w][2] (dx,dy)/4
     __half* flows_b4 = nullptr;
     __half* mask_in4 = nullptr;   // [T][h][w] fp16
-    __half* mask_upd4 = nullptr;
     size_t arena_mark = 0;
     std::vector<int> ring_idx_host;
     int* ring_idx = nullptr;      // [n_win][193]
-    int* win_flags = nullptr;     // [n_win]
     int gh = 0, gw = 0, nh = 0, nw = 0, ph = 0, pw = 0;
   } gen;
   // multi-GPU (comm.cu): NCCL communicator (ncclComm_t, opaque here) of this engine's process group
@@ -117,20 +115,21 @@ struct PPConvCall {
   PPConvCall(PPEngine& e, const std::string& name, int N, int H, int W);
   PPConvCall& in(const __half* ptr, int cs, int co, int channels, int gstep = 0);
   PPConvCall& geom(int sh, int sw, int ph, int pw, int dh = 1, int dw = 1, int replicate = 0);
-  PPConvCall& out(void* ptr, int cs, int co, int fp32 = 0, int gstep = 0);
+  PPConvCall& out(__half* ptr, int cs, int co, int gstep = 0);
+  PPConvCall& out_f32(float* ptr, int cs, int co);   // plain fp32 [pix][cs] output of either form
   PPConvCall& act(int act1, float slope = 0.f, float scale = 1.f, int act2 = PP_ACT_NONE);
   PPConvCall& residual(const __half* ptr, int cs, int co);
   PPConvCall& gru_zr(const __half* h, int h_cs, int h_co, __half* rh, int rh_cs, int rh_co);
   PPConvCall& gru_h(const __half* h, int h_cs, int h_co, const __half* z, int z_cs, int z_co);
-  // Split-tf32 form (PPConvParams::split, conv_igemm.cuh): the weights must have been registered as a split image.  Every
-  // tensor is an fp32 [pix][hi C | lo C] pair tensor given by its pointer and real channel count C; `co` / `channels` count
-  // fp32 channels.  The input segments added with in_split are read as (hi..., lo..., hi...) by run().
-  PPConvCall& tf32();
-  PPConvCall& in_split(const float* ptr, int C, int co, int channels);
-  PPConvCall& out_split(float* ptr, int C, int co);
-  PPConvCall& residual_split(const float* ptr, int C, int co);
-  PPConvCall& gru_zr_split(const float* h, int h_C, int h_co, float* rh, int rh_C, int rh_co);
-  PPConvCall& gru_h_split(const float* h, int h_C, int h_co, const float* z, int z_C, int z_co);
+  // Split-tf32 form (PPConvParams::split, conv_igemm.cuh): the float* overloads.  A float* input puts the call in this
+  // form; the weights must have been registered as a split image and every input must then be a float* one.  Every
+  // tensor is an fp32 [pix][hi C | lo C] pair tensor given by its pointer and real channel count C; `co` / `channels`
+  // count fp32 channels.  The inputs are read as (hi..., lo..., hi...) segments by run().
+  PPConvCall& in(const float* ptr, int C, int co, int channels);
+  PPConvCall& out(float* ptr, int C, int co);
+  PPConvCall& residual(const float* ptr, int C, int co);
+  PPConvCall& gru_zr(const float* h, int h_C, int h_co, float* rh, int rh_C, int rh_co);
+  PPConvCall& gru_h(const float* h, int h_C, int h_co, const float* z, int z_C, int z_co);
   int run(cudaStream_t st);
 
  private:
@@ -149,28 +148,34 @@ int pp_comm_all_gather_blocks_impl(PPEngine& e, void* buf, const long long* row_
                                    size_t row_bytes, int first_rank, int n_members, cudaStream_t st);
 
 // ---- stages ---------------------------------------------------------------------------------------
-// fp32: the split-tf32 path (weights registered under "<name>.tf32", see engine.py); otherwise fp16 activations
+// The stages that exist in two precisions are templates on the element type E of their activations, instantiated for
+// __half (fp16) and float (the node's fp16="disable"); the C entry points (capi.cu) choose it.
+// RAFT, E = float: the split-tf32 path, weights registered under "<name>.tf32" (engine.py).
+template <class E>
 int pp_stage_raft(PPEngine& e, const float* frames, int T, int H, int W, int iters, float* flows_f, float* flows_b,
-                  bool fp32, cudaStream_t st);
+                  cudaStream_t st);
 // RAFT correlation pyramid (raft.cu), shared by pp_stage_raft and pp_op_corr_pyramid.  P_pad: rows of a packed fmap
-// (pp_k_pack_b_operand / _split) of P pixels.
+// (pp_k_pack_b_operand) of P pixels.
 int pp_raft_corr_pad(int P);
 // All-pairs correlation of `pairs` frame pairs, scaled by 1/sqrt(256): group g correlates fmap g after fmap1 (fp16
 // [P][256], or fp32 split [P][hi 256 | lo 256]) with packed fmap g after fpack2 into corr0 + g*P*P (fp16 / fp32).
-int pp_raft_corr_volume(PPEngine& e, const void* fmap1, const void* fpack2, int pairs, int P, int P_pad, bool fp32,
-                        void* corr0, cudaStream_t st);
+template <class E>
+int pp_raft_corr_volume(PPEngine& e, const E* fmap1, const E* fpack2, int pairs, int P, int P_pad, E* corr0,
+                        cudaStream_t st);
 // Levels 1..3 from level 0: 2x2 average pooling of each of the M query maps of h8 x w8
-int pp_raft_corr_pool(PPEngine& e, void* const corr[4], long long M, int h8, int w8, bool fp32, cudaStream_t st);
+template <class E>
+int pp_raft_corr_pool(PPEngine& e, E* const corr[4], long long M, int h8, int w8, cudaStream_t st);
 int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
                            int H, int W, float* out_f, float* out_b, int team_first, int team_size, cudaStream_t st);
-// fp32: frames / masks stored as float4 and flows as float2 (the node's fp16="disable"), else 4 x fp16 / __half2
+// E = float: frames / masks stored as float4 and flows as float2, E = __half: 4 x fp16 / __half2
+template <class E>
 int pp_stage_image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f,
-                             const float* flows_b, int T, int H, int W, float* upd_frames, float* upd_masks, bool fp32,
+                             const float* flows_b, int T, int H, int W, float* upd_frames, float* upd_masks,
                              cudaStream_t st);
 int pp_stage_gen_begin(PPEngine& e, const float* frames, const float* masks_in, const float* masks_upd,
                  const float* flows_f, const float* flows_b, int T, int H, int W, const unsigned char* need,
                  cudaStream_t st);
-int pp_stage_gen_window(PPEngine& e, const int* frame_ids, int t, int l_t, __half* pred /*[l_t][H][W][8]*/,
+int pp_stage_gen_window(PPEngine& e, const int* frame_ids, int t, int l_t, __half* pred /*[l_t][H][W][4]*/,
                   cudaStream_t st);
 int pp_stage_gen_run(PPEngine& e, const int* frame_ids, const int* win_t, const int* win_lt, int n_windows,
                      __half* pred /*[sum l_t][H][W][4]*/, cudaStream_t st);

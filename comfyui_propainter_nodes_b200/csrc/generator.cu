@@ -2,8 +2,8 @@
 //
 // Session API: pp_gen_begin() encodes every frame ONCE (the reference re-encodes a frame in every sliding
 // window it appears in; the encoder is per-frame, so caching is result-identical) and down-samples flows and
-// masks once; pp_gen_window() then runs feature propagation + transformer + decoder for one window given
-// frame indices into the session.
+// masks once; pp_gen_run() then runs feature propagation + transformer + decoder for all sliding windows of the clip
+// in one batched pass (pp_gen_window(): for a single window), given frame indices into the session.
 #include <string.h>
 
 #include "engine.cuh"
@@ -84,10 +84,8 @@ int pp_stage_gen_begin(PPEngine& e, const float* frames, const float* masks_in, 
   PP_TRY(pp_alloc(e, &g.flows_f4, (size_t)(T - 1) * P4 * 2, "flows_f/4"));
   PP_TRY(pp_alloc(e, &g.flows_b4, (size_t)(T - 1) * P4 * 2, "flows_b/4"));
   PP_TRY(pp_alloc(e, &g.mask_in4, (size_t)T * P4 * 8, "mask2/4"));
-  g.mask_upd4 = nullptr;
   const int n_win = (g.nh / WIN_H) * (g.nw / WIN_W);
   PP_TRY(pp_alloc(e, &g.ring_idx, (size_t)n_win * RING, "ring indices"));
-  PP_TRY(pp_alloc(e, &g.win_flags, (size_t)n_win, "window flags"));
   pp_build_ring_indices(g.nh, g.nw, g.ring_idx_host);
   PP_CUDA_CHECK(cudaMemcpyAsync(g.ring_idx, g.ring_idx_host.data(), g.ring_idx_host.size() * sizeof(int),
                                 cudaMemcpyHostToDevice, st));
@@ -138,9 +136,9 @@ int pp_stage_gen_begin(PPEngine& e, const float* frames, const float* masks_in, 
     // input = cat(frame[3], mask_in[1], mask_updated[1]) (propainter.py:374-383), padded to 8 channels
     for (const Run& r : runs) {
       __half* dst = x8 + (size_t)r.slot * HW * 8;
-      PP_TRY(pp_k_nchw_f32_to_nhwc_f16(frames + (size_t)r.frame * 3 * HW, dst, r.len, 3, H, W, 8, 0, 8, st));
-      PP_TRY(pp_k_nchw_f32_to_nhwc_f16(masks_in + (size_t)r.frame * HW, dst, r.len, 1, H, W, 8, 3, 1, st));
-      PP_TRY(pp_k_nchw_f32_to_nhwc_f16(masks_upd + (size_t)r.frame * HW, dst, r.len, 1, H, W, 8, 4, 1, st));
+      PP_TRY(pp_k_nchw_to_act(frames + (size_t)r.frame * 3 * HW, dst, r.len, 3, H, W, 8, st));
+      PP_TRY(pp_k_nchw_to_act(masks_in + (size_t)r.frame * HW, dst, r.len, 1, H, W, 8, st, 3, 1));
+      PP_TRY(pp_k_nchw_to_act(masks_upd + (size_t)r.frame * HW, dst, r.len, 1, H, W, 8, st, 4, 1));
       e.launches += 3;
     }
     __half* enc_out = (runs.size() == 1) ? g.enc + (size_t)runs[0].frame * P4 * 128 : enc_tmp;
@@ -152,9 +150,9 @@ int pp_stage_gen_begin(PPEngine& e, const float* frames, const float* masks_in, 
     PP_TRY(PPConvCall(e, "gen.encoder.8", n, h4, w4).in(x0, 256, 0, 256).out(b8, 384, 0).act(PP_ACT_LRELU, s).run(st));
     // grouped layers: group k sees cat(x0[k-th slice], out[k-th slice]) (propainter.py:268-273)
     PP_TRY(PPConvCall(e, "gen.encoder.10", n, h4, w4).in(x0, 256, 0, 128, 128).in(b8, 384, 0, 192, 192)
-               .out(b10, 512, 0, 0, 256).act(PP_ACT_LRELU, s).run(st));
+               .out(b10, 512, 0, 256).act(PP_ACT_LRELU, s).run(st));
     PP_TRY(PPConvCall(e, "gen.encoder.12", n, h4, w4).in(x0, 256, 0, 64, 64).in(b10, 512, 0, 128, 128)
-               .out(b12, 384, 0, 0, 96).act(PP_ACT_LRELU, s).run(st));
+               .out(b12, 384, 0, 96).act(PP_ACT_LRELU, s).run(st));
     // 8 groups of 80 -> 32 channels: dense block-diagonal weights (engine.py), one launch on the halo kernel
     PP_TRY(PPConvCall(e, "gen.encoder.14", n, h4, w4).in(x0, 256, 0, 256).in(b12, 384, 0, 384)
                .out(b14, 256, 0).act(PP_ACT_LRELU, s).run(st));

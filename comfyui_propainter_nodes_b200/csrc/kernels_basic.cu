@@ -19,15 +19,6 @@ __global__ void nchw_f32_to_nhwc_f16(const float* __restrict__ src, __half* __re
   for (int c = C; c < zero_to; ++c) d[c] = __float2half_rn(0.f);
 }
 
-__global__ void nhwc_f16_to_nchw_f32(const __half* __restrict__ src, int src_cs, int src_co, float* __restrict__ dst,
-                                     int C, long long HW, long long npix) {
-  long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (p >= npix) return;
-  const long long n = p / HW, hw = p - n * HW;
-  const __half* s = src + p * src_cs + src_co;
-  for (int c = 0; c < C; ++c) dst[(n * C + c) * HW + hw] = __half2float(s[c]);
-}
-
 // Bilinear x2 upsample, align_corners=True (reference deconv: F.interpolate(scale_factor=2, 'bilinear', True)).
 // One thread per (2x2 block of output pixels, 8-channel vector).  With scale (H-1)/(2H-1) < 1/2 the outputs of block
 // (r, c) interpolate between input rows (r-1, r) / (r, r+1) and columns (c-1, c) / (c, c+1): interior blocks load and
@@ -98,16 +89,6 @@ __global__ void __launch_bounds__(256) upsample2x_ac(const __half* __restrict__ 
     }
 }
 
-__global__ void copy_channels(const __half* __restrict__ src, int src_cs, int src_co, __half* __restrict__ dst,
-                              int dst_cs, int dst_co, long long npix, int C8) {
-  long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (idx >= npix * C8) return;
-  const int c8 = idx % C8;
-  const long long p = idx / C8;
-  *reinterpret_cast<uint4*>(dst + p * dst_cs + dst_co + c8 * 8) =
-      *reinterpret_cast<const uint4*>(src + p * src_cs + src_co + c8 * 8);
-}
-
 // dst block j <- src block idx[j]; blocks are `block16` 16-byte units (frame-sized gathers for window batching)
 __global__ void gather_blocks(uint4* __restrict__ dst, const uint4* __restrict__ src, const int* __restrict__ idx,
                               long long n, long long block16) {
@@ -126,28 +107,14 @@ __global__ void copy_blocks(uint4* __restrict__ dst, const int* __restrict__ dst
   dst[(long long)dst_idx[j] * block16 + u] = src[(long long)src_idx[j] * block16 + u];
 }
 
-__global__ void fill_f16(__half* dst, long long n, float v) {
-  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = __float2half_rn(v);
-}
-
 }  // namespace
 
-int pp_k_nchw_f32_to_nhwc_f16(const float* src, __half* dst, int N, int C, int H, int W, int dst_cs, int dst_co,
-                              int zero_fill_to, cudaStream_t st) {
+int pp_k_nchw_to_act(const float* src, __half* dst, int N, int C, int H, int W, int cs, cudaStream_t st, int dst_co,
+                     int zero_fill_to) {
   const long long npix = (long long)N * H * W;
   if (npix == 0) return PP_OK;
-  nchw_f32_to_nhwc_f16<<<nblocks(npix), TPB, 0, st>>>(src, dst, C, (long long)H * W, npix, dst_cs, dst_co,
-                                                       zero_fill_to);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_nhwc_f16_to_nchw_f32(const __half* src, int src_cs, int src_co, float* dst, int N, int C, int H, int W,
-                              cudaStream_t st) {
-  const long long npix = (long long)N * H * W;
-  if (npix == 0) return PP_OK;
-  nhwc_f16_to_nchw_f32<<<nblocks(npix), TPB, 0, st>>>(src, src_cs, src_co, dst, C, (long long)H * W, npix);
+  nchw_f32_to_nhwc_f16<<<nblocks(npix), TPB, 0, st>>>(src, dst, C, (long long)H * W, npix, cs, dst_co,
+                                                       zero_fill_to < 0 ? cs - dst_co : zero_fill_to);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
@@ -160,16 +127,6 @@ int pp_k_upsample2x(const __half* src, int src_cs, int src_co, __half* dst, int 
   PP_REQUIRE(H <= 65535 && N <= 65535, "upsample2x: %d rows / %d images exceed the grid limits", H, N);
   const dim3 grid(pp_ceil_div(W * (C / 8), 256), H, N);
   upsample2x_ac<<<grid, 256, 0, st>>>(src, src_cs, src_co, dst, dst_cs, dst_co, H, W, C / 8);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_copy_channels(const __half* src, int src_cs, int src_co, __half* dst, int dst_cs, int dst_co, long long npix,
-                       int C, cudaStream_t st) {
-  PP_REQUIRE(C % 8 == 0 && src_cs % 8 == 0 && dst_cs % 8 == 0 && src_co % 8 == 0 && dst_co % 8 == 0,
-             "copy_channels: channels must be multiples of 8");
-  if (npix == 0) return PP_OK;
-  copy_channels<<<nblocks(npix * (C / 8)), TPB, 0, st>>>(src, src_cs, src_co, dst, dst_cs, dst_co, npix, C / 8);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
@@ -192,13 +149,6 @@ int pp_k_copy_blocks(void* dst, const int* dst_idx_dev, const void* src, const i
   const long long b16 = block_bytes / 16;
   copy_blocks<<<nblocks(n * b16), TPB, 0, st>>>(static_cast<uint4*>(dst), dst_idx_dev, static_cast<const uint4*>(src),
                                                  src_idx_dev, n, b16);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_fill_f16(__half* dst, long long n, float v, cudaStream_t st) {
-  if (n == 0) return PP_OK;
-  fill_f16<<<nblocks(n), TPB, 0, st>>>(dst, n, v);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }

@@ -2,6 +2,8 @@
 // modulated deformable sampling, flow-completion pack/combine, 1/4 downsampling.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "kernels.cuh"
 #include "conv_igemm.cuh"
 #include "dcn_sample.cuh"
@@ -114,6 +116,10 @@ struct ImgF32 {
   __device__ static Pix make(float r, float g, float b, float m) { return make_float4(r, g, b, m); }
   __device__ static Flow make_flow(float x, float y) { return make_float2(x, y); }
 };
+
+// storage type of a launcher's element type (__half / float)
+template <class E>
+using ImgOf = std::conditional_t<sizeof(E) == 4, ImgF32, ImgF16>;
 
 template <class S>
 __device__ __forceinline__ float fb_valid_of(float2 fp, const typename S::Flow* fchk, const Bilin& b, int W) {
@@ -516,21 +522,27 @@ __global__ void downsample_mask4(const float* __restrict__ src, __half* __restri
   dst[idx * dst_cs + dst_co] = __float2half_rn(src[((long long)i * H + 4 * y) * W + 4 * x]);
 }
 
-template <class S>
-int imgprop_step_launch(const void* cur, const void* prop_in, void* prop_out, const void* flow_prop,
-                        const void* flow_check, int H, int W, cudaStream_t st) {
+}  // namespace
+
+template <class E>
+int pp_k_imgprop_step(const E* cur, const E* prop_in, E* prop_out, const E* flow_prop, const E* flow_check, int H,
+                      int W, cudaStream_t st) {
+  using S = ImgOf<E>;
   using Pix = typename S::Pix;
   using Flow = typename S::Flow;
   imgprop_step<S><<<nblocks((long long)H * W), TPB, 0, st>>>(
-      static_cast<const Pix*>(cur), static_cast<const Pix*>(prop_in), static_cast<Pix*>(prop_out),
-      static_cast<const Flow*>(flow_prop), static_cast<const Flow*>(flow_check), H, W);
+      reinterpret_cast<const Pix*>(cur), reinterpret_cast<const Pix*>(prop_in), reinterpret_cast<Pix*>(prop_out),
+      reinterpret_cast<const Flow*>(flow_prop), reinterpret_cast<const Flow*>(flow_check), H, W);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
+template int pp_k_imgprop_step(const __half*, const __half*, __half*, const __half*, const __half*, int, int, cudaStream_t);
+template int pp_k_imgprop_step(const float*, const float*, float*, const float*, const float*, int, int, cudaStream_t);
 
-template <class S>
-int imgprop_run(const void* in4, void* bwd, void* fwd, const void* ff, const void* fbk, const float* masks, int T,
-                int H, int W, int* scratch, cudaStream_t st) {
+template <class E>
+int pp_k_imgprop_run(const E* in4, E* bwd, E* fwd, const E* ff, const E* fbk, const float* masks, int T, int H, int W,
+                     int* scratch, cudaStream_t st) {
+  using S = ImgOf<E>;
   static int grid_max = 0;      // one per storage type: the fp32 kernel has its own register footprint
   if (grid_max == 0) {
     int sms = 0, per_sm = 0;
@@ -547,93 +559,57 @@ int imgprop_run(const void* in4, void* bwd, void* fwd, const void* ff, const voi
   PP_CUDA_CHECK(cudaGetLastError());
   using Pix = typename S::Pix;
   using Flow = typename S::Flow;
-  const Pix* a0 = static_cast<const Pix*>(in4);
-  Pix* a1 = static_cast<Pix*>(bwd);
-  Pix* a2 = static_cast<Pix*>(fwd);
-  const Flow* a3 = static_cast<const Flow*>(ff);
-  const Flow* a4 = static_cast<const Flow*>(fbk);
+  const Pix* a0 = reinterpret_cast<const Pix*>(in4);
+  Pix* a1 = reinterpret_cast<Pix*>(bwd);
+  Pix* a2 = reinterpret_cast<Pix*>(fwd);
+  const Flow* a3 = reinterpret_cast<const Flow*>(ff);
+  const Flow* a4 = reinterpret_cast<const Flow*>(fbk);
   const int* a8 = scratch;
   unsigned int* a9 = reinterpret_cast<unsigned int*>(scratch + 4);
   void* args[] = {&a0, &a1, &a2, &a3, &a4, &T, &H, &W, &a8, &a9};
   PP_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)imgprop_persistent<S>, dim3(grid_max), dim3(256), args, 0, st));
   return PP_OK;
 }
+template int pp_k_imgprop_run(const __half*, __half*, __half*, const __half*, const __half*, const float*, int, int, int,
+                              int*, cudaStream_t);
+template int pp_k_imgprop_run(const float*, float*, float*, const float*, const float*, const float*, int, int, int, int*,
+                              cudaStream_t);
 
-template <class S>
-int imgprop_pack_launch(const float* frames, const float* masks, void* dst, int T, int H, int W, cudaStream_t st) {
+template <class E>
+int pp_k_imgprop_pack(const float* frames, const float* masks, E* dst, int T, int H, int W, cudaStream_t st) {
+  using S = ImgOf<E>;
   const long long HW = (long long)H * W, total = HW * T;
-  imgprop_pack<S><<<nblocks(total), TPB, 0, st>>>(frames, masks, static_cast<typename S::Pix*>(dst), HW, total);
+  imgprop_pack<S><<<nblocks(total), TPB, 0, st>>>(frames, masks, reinterpret_cast<typename S::Pix*>(dst), HW, total);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
+template int pp_k_imgprop_pack(const float*, const float*, __half*, int, int, int, cudaStream_t);
+template int pp_k_imgprop_pack(const float*, const float*, float*, int, int, int, cudaStream_t);
 
-template <class S>
-int imgprop_finish_launch(const void* prop, const float* frames, const float* masks, float* upd_frames,
-                          float* upd_masks, int T, int H, int W, cudaStream_t st) {
+template <class E>
+int pp_k_imgprop_finish(const E* prop, const float* frames, const float* masks, float* upd_frames, float* upd_masks,
+                        int T, int H, int W, cudaStream_t st) {
+  using S = ImgOf<E>;
   const long long HW = (long long)H * W, total = HW * T;
-  imgprop_finish<S><<<nblocks(total), TPB, 0, st>>>(static_cast<const typename S::Pix*>(prop), frames, masks,
+  imgprop_finish<S><<<nblocks(total), TPB, 0, st>>>(reinterpret_cast<const typename S::Pix*>(prop), frames, masks,
                                                     upd_frames, upd_masks, HW, total);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
+template int pp_k_imgprop_finish(const __half*, const float*, const float*, float*, float*, int, int, int, cudaStream_t);
+template int pp_k_imgprop_finish(const float*, const float*, const float*, float*, float*, int, int, int, cudaStream_t);
 
-template <class S>
-int flow_to_nhwc2_launch(const float* src, void* dst, int n, int H, int W, cudaStream_t st) {
+template <class E>
+int pp_k_flow_to_nhwc2(const float* src, E* dst, int n, int H, int W, cudaStream_t st) {
+  using S = ImgOf<E>;
   const long long HW = (long long)H * W, total = HW * n;
   if (total == 0) return PP_OK;
-  flow_to_nhwc2<S><<<nblocks(total), TPB, 0, st>>>(src, static_cast<typename S::Flow*>(dst), HW, total);
+  flow_to_nhwc2<S><<<nblocks(total), TPB, 0, st>>>(src, reinterpret_cast<typename S::Flow*>(dst), HW, total);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
-
-}  // namespace
-
-int pp_k_imgprop_step(const __half* cur, const __half* prop_in, __half* prop_out, const __half* flow_prop,
-                      const __half* flow_check, int H, int W, cudaStream_t st) {
-  return imgprop_step_launch<ImgF16>(cur, prop_in, prop_out, flow_prop, flow_check, H, W, st);
-}
-
-int pp_k_imgprop_step_f32(const float* cur, const float* prop_in, float* prop_out, const float* flow_prop,
-                          const float* flow_check, int H, int W, cudaStream_t st) {
-  return imgprop_step_launch<ImgF32>(cur, prop_in, prop_out, flow_prop, flow_check, H, W, st);
-}
-
-// bwd / fwd must hold copies of in4; scratch = 8 ints (bbox[4], barrier counter, pad)
-int pp_k_imgprop_run(const __half* in4, __half* bwd, __half* fwd, const __half* ff, const __half* fbk,
-                     const float* masks, int T, int H, int W, int* scratch, cudaStream_t st) {
-  return imgprop_run<ImgF16>(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st);
-}
-
-int pp_k_imgprop_run_f32(const float* in4, float* bwd, float* fwd, const float* ff, const float* fbk,
-                         const float* masks, int T, int H, int W, int* scratch, cudaStream_t st) {
-  return imgprop_run<ImgF32>(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st);
-}
-
-int pp_k_imgprop_pack(const float* frames, const float* masks, __half* dst, int T, int H, int W, cudaStream_t st) {
-  return imgprop_pack_launch<ImgF16>(frames, masks, dst, T, H, W, st);
-}
-
-int pp_k_imgprop_pack_f32(const float* frames, const float* masks, float* dst, int T, int H, int W, cudaStream_t st) {
-  return imgprop_pack_launch<ImgF32>(frames, masks, dst, T, H, W, st);
-}
-
-int pp_k_imgprop_finish(const __half* prop, const float* frames, const float* masks, float* upd_frames,
-                        float* upd_masks, int T, int H, int W, cudaStream_t st) {
-  return imgprop_finish_launch<ImgF16>(prop, frames, masks, upd_frames, upd_masks, T, H, W, st);
-}
-
-int pp_k_imgprop_finish_f32(const float* prop, const float* frames, const float* masks, float* upd_frames,
-                            float* upd_masks, int T, int H, int W, cudaStream_t st) {
-  return imgprop_finish_launch<ImgF32>(prop, frames, masks, upd_frames, upd_masks, T, H, W, st);
-}
-
-int pp_k_flow_to_nhwc2(const float* src, __half* dst, int n, int H, int W, cudaStream_t st) {
-  return flow_to_nhwc2_launch<ImgF16>(src, dst, n, H, W, st);
-}
-
-int pp_k_flow_to_nhwc2_f32(const float* src, float* dst, int n, int H, int W, cudaStream_t st) {
-  return flow_to_nhwc2_launch<ImgF32>(src, dst, n, H, W, st);
-}
+template int pp_k_flow_to_nhwc2(const float*, __half*, int, int, int, cudaStream_t);
+template int pp_k_flow_to_nhwc2(const float*, float*, int, int, int, cudaStream_t);
 
 int pp_k_rfc_pack_input(const float* flows, const float* masks, __half* dst, long long dst_tstride_pix, int T, int H,
                         int W, int reverse_time, cudaStream_t st) {

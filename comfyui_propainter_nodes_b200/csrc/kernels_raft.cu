@@ -452,22 +452,9 @@ size_t pp_k_instnorm_scratch_floats(int N, int HW, int C) {
 }
 
 // sums: scratch of pp_k_instnorm_scratch_floats(N, HW, C) floats; the statistics [N][2][C] are its first N*2*C entries
-int pp_k_instnorm_stats(const __half* x, int N, int HW, int C, float* sums, cudaStream_t st) {
-  PP_REQUIRE(C % 2 == 0 && C <= 256, "instnorm: unsupported C=%d", C);
-  const int pix_per_block = 1024;
-  const int nblk = pp_ceil_div(HW, pix_per_block);
-  float* partial = sums + (size_t)N * 2 * C;
-  unsigned int* counters = reinterpret_cast<unsigned int*>(partial + (size_t)N * nblk * 2 * C);
-  PP_CUDA_CHECK(cudaMemsetAsync(counters, 0, (size_t)N * sizeof(unsigned int), st));
-  dim3 grid(nblk, N);
-  const int lanes = 256 / (C / 2);
-  instnorm_stats<false><<<grid, 256, (size_t)lanes * 2 * C * sizeof(float), st>>>(x, HW, C, sums, partial, counters,
-                                                                                  pix_per_block, 0);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_instnorm_stats_f32(const float* x, int N, int HW, int C, float* sums, cudaStream_t st) {
+template <class E>
+int pp_k_instnorm_stats(const E* x, int N, int HW, int C, float* sums, cudaStream_t st) {
+  constexpr bool F32 = sizeof(E) == 4;
   PP_REQUIRE(C % 2 == 0 && C <= 256, "instnorm: unsupported C=%d", C);
   const int pix_per_block = 1024;
   const int nblk = pp_ceil_div(HW, pix_per_block);
@@ -475,34 +462,31 @@ int pp_k_instnorm_stats_f32(const float* x, int N, int HW, int C, float* sums, c
   unsigned int* counters = reinterpret_cast<unsigned int*>(partial + (size_t)N * nblk * 2 * C);
   dim3 grid(nblk, N);
   const int lanes = 256 / (C / 2);
-  for (int centred = 0; centred < 2; ++centred) {   // sums of x, then sums of (x - mean)^2
+  for (int centred = 0; centred < (F32 ? 2 : 1); ++centred) {   // fp32: sums of x, then sums of (x - mean)^2
     PP_CUDA_CHECK(cudaMemsetAsync(counters, 0, (size_t)N * sizeof(unsigned int), st));
-    instnorm_stats<true><<<grid, 256, (size_t)lanes * 2 * C * sizeof(float), st>>>(x, HW, C, sums, partial, counters,
-                                                                                   pix_per_block, centred);
+    instnorm_stats<F32><<<grid, 256, (size_t)lanes * 2 * C * sizeof(float), st>>>(x, HW, C, sums, partial, counters,
+                                                                                  pix_per_block, centred);
     PP_CUDA_CHECK(cudaGetLastError());
   }
   return PP_OK;
 }
+template int pp_k_instnorm_stats(const __half*, int, int, int, float*, cudaStream_t);
+template int pp_k_instnorm_stats(const float*, int, int, int, float*, cudaStream_t);
 
-int pp_k_instnorm_apply(const __half* x, const float* sums, const __half* residual, __half* out, int N, int HW, int C,
-                        int relu, cudaStream_t st) {
+template <class E>
+int pp_k_instnorm_apply(const E* x, const float* sums, const E* residual, E* out, int N, int HW, int C, int relu,
+                        cudaStream_t st) {
   if ((long long)N * HW == 0) return PP_OK;
   PP_REQUIRE(N <= 65535 && (long long)HW * (C / 2) < (1LL << 31), "instnorm: %d images of %d pixels exceed the grid limits", N, HW);
-  instnorm_apply<false><<<dim3(pp_ceil_div(HW * (C / 2), 256), N), 256, 0, st>>>(x, sums, residual, out, HW, C, relu);
+  instnorm_apply<sizeof(E) == 4><<<dim3(pp_ceil_div(HW * (C / 2), 256), N), 256, 0, st>>>(x, sums, residual, out, HW, C,
+                                                                                          relu);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
+template int pp_k_instnorm_apply(const __half*, const float*, const __half*, __half*, int, int, int, int, cudaStream_t);
+template int pp_k_instnorm_apply(const float*, const float*, const float*, float*, int, int, int, int, cudaStream_t);
 
-int pp_k_instnorm_apply_f32(const float* x, const float* sums, const float* residual, float* out, int N, int HW, int C,
-                            int relu, cudaStream_t st) {
-  if ((long long)N * HW == 0) return PP_OK;
-  PP_REQUIRE(N <= 65535 && (long long)HW * (C / 2) < (1LL << 31), "instnorm: %d images of %d pixels exceed the grid limits", N, HW);
-  instnorm_apply<true><<<dim3(pp_ceil_div(HW * (C / 2), 256), N), 256, 0, st>>>(x, sums, residual, out, HW, C, relu);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_nchw_f32_to_split(const float* src, float* dst, int N, int C, int H, int W, int cs, cudaStream_t st) {
+int pp_k_nchw_to_act(const float* src, float* dst, int N, int C, int H, int W, int cs, cudaStream_t st) {
   PP_REQUIRE(C <= cs && cs % 4 == 0, "nchw_to_split: C=%d cs=%d", C, cs);
   const long long total = (long long)N * H * W * cs;
   if (total == 0) return PP_OK;
@@ -511,7 +495,7 @@ int pp_k_nchw_f32_to_split(const float* src, float* dst, int N, int C, int H, in
   return PP_OK;
 }
 
-int pp_k_pack_b_operand_split(const float* src, float* dst, int G, int R, int R_pad, int K, cudaStream_t st) {
+int pp_k_pack_b_operand(const float* src, float* dst, int G, int R, int R_pad, int K, cudaStream_t st) {
   PP_REQUIRE(K % 32 == 0 && R_pad % 8 == 0, "pack_b_operand_split: K=%d must be a multiple of 32", K);
   const long long total = (long long)G * R_pad * (3 * K / 4);
   pack_b_operand_split<<<nblocks(total), TPB, 0, st>>>(src, dst, R, R_pad, K, total);
@@ -527,52 +511,40 @@ int pp_k_pack_b_operand(const __half* src, __half* dst, int G, int R, int R_pad,
   return PP_OK;
 }
 
-int pp_k_corr_pool(const __half* src, __half* dst, long long nq, int h, int w, cudaStream_t st) {
+template <class E>
+int pp_k_corr_pool(const E* src, E* dst, long long nq, int h, int w, cudaStream_t st) {
   if (nq * (h / 2) * (w / 2) == 0) return PP_OK;
   PP_REQUIRE(nq < (1LL << 31), "corr_pool: too many query maps");
-  corr_pool<__half><<<(unsigned)nq, 128, 0, st>>>(src, dst, h, w);
+  corr_pool<E><<<(unsigned)nq, 128, 0, st>>>(src, dst, h, w);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
+template int pp_k_corr_pool(const __half*, __half*, long long, int, int, cudaStream_t);
+template int pp_k_corr_pool(const float*, float*, long long, int, int, cudaStream_t);
 
-int pp_k_corr_pool_f32(const float* src, float* dst, long long nq, int h, int w, cudaStream_t st) {
-  if (nq * (h / 2) * (w / 2) == 0) return PP_OK;
-  PP_REQUIRE(nq < (1LL << 31), "corr_pool: too many query maps");
-  corr_pool<float><<<(unsigned)nq, 128, 0, st>>>(src, dst, h, w);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_corr_lookup(const __half* l0, const __half* l1, const __half* l2, const __half* l3, const float* coords,
-                     __half* out, int out_cs, long long nq, int P, int h8, int w8, cudaStream_t st) {
-  PP_REQUIRE(out_cs >= 324 && out_cs <= 352, "corr_lookup: out_cs=%d not in [324,352]", out_cs);
-  CorrLevels<__half> lv;
-  lv.p[0] = l0; lv.p[1] = l1; lv.p[2] = l2; lv.p[3] = l3;
-  (void)P;
-  corr_lookup<__half><<<(unsigned)((nq + LOOKUP_WARPS - 1) / LOOKUP_WARPS), LOOKUP_WARPS * 32, 0, st>>>(lv, coords, out,
-                                                                                                      out_cs, nq, h8, w8);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_corr_lookup_f32(const float* l0, const float* l1, const float* l2, const float* l3, const float* coords,
-                         float* out, int out_C, long long nq, int h8, int w8, cudaStream_t st) {
+template <class E>
+int pp_k_corr_lookup(const E* l0, const E* l1, const E* l2, const E* l3, const float* coords, E* out, int out_C,
+                     long long nq, int h8, int w8, cudaStream_t st) {
   PP_REQUIRE(out_C >= 324 && out_C <= 352, "corr_lookup: out_C=%d not in [324,352]", out_C);
-  CorrLevels<float> lv;
+  CorrLevels<E> lv;
   lv.p[0] = l0; lv.p[1] = l1; lv.p[2] = l2; lv.p[3] = l3;
-  corr_lookup<float><<<(unsigned)((nq + LOOKUP_WARPS - 1) / LOOKUP_WARPS), LOOKUP_WARPS * 32, 0, st>>>(lv, coords, out,
-                                                                                                     out_C, nq, h8, w8);
+  corr_lookup<E><<<(unsigned)((nq + LOOKUP_WARPS - 1) / LOOKUP_WARPS), LOOKUP_WARPS * 32, 0, st>>>(lv, coords, out,
+                                                                                                 out_C, nq, h8, w8);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+template int pp_k_corr_lookup(const __half*, const __half*, const __half*, const __half*, const float*, __half*, int,
+                              long long, int, int, cudaStream_t);
+template int pp_k_corr_lookup(const float*, const float*, const float*, const float*, const float*, float*, int,
+                              long long, int, int, cudaStream_t);
+
+int pp_k_cnet_split(const __half* c, __half* hx, int hx_C, long long npix, cudaStream_t st) {
+  cnet_split<<<nblocks(npix * 256), TPB, 0, st>>>(c, hx, hx_C, npix * 256);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
 
-int pp_k_cnet_split(const __half* c, __half* hx, int hx_cs, long long npix, cudaStream_t st) {
-  cnet_split<<<nblocks(npix * 256), TPB, 0, st>>>(c, hx, hx_cs, npix * 256);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_cnet_split_f32(const float* c, float* hx, int hx_C, long long npix, cudaStream_t st) {
+int pp_k_cnet_split(const float* c, float* hx, int hx_C, long long npix, cudaStream_t st) {
   cnet_split_f32<<<nblocks(npix * 256), TPB, 0, st>>>(c, hx, hx_C, npix * 256);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
@@ -612,7 +584,7 @@ int pp_k_flow_patch7x7(const __half* flow8, __half* out, int B, int h8, int w8, 
   return PP_OK;
 }
 
-int pp_k_flow_patch7x7_f32(const float* coords1, float* out, int B, int h8, int w8, cudaStream_t st) {
+int pp_k_flow_patch7x7(const float* coords1, float* out, int B, int h8, int w8, cudaStream_t st) {
   const long long total = (long long)B * h8 * w8 * 128;
   if (total == 0) return PP_OK;
   flow_patch7x7_f32<<<nblocks(total), TPB, 0, st>>>(coords1, out, h8, w8, total);
@@ -620,8 +592,8 @@ int pp_k_flow_patch7x7_f32(const float* coords1, float* out, int B, int h8, int 
   return PP_OK;
 }
 
-int pp_k_raft_coords_f32(const float* delta, float* coords1, float* hx, int hx_C, int hx_flow_co, int B, int h8, int w8,
-                         cudaStream_t st) {
+int pp_k_raft_coords(const float* delta, float* coords1, float* hx, int hx_C, int hx_flow_co, int B, int h8, int w8,
+                     cudaStream_t st) {
   const long long total = (long long)B * h8 * w8;
   raft_coords_f32<<<nblocks(total), TPB, 0, st>>>(delta, coords1, hx, hx_C, hx_flow_co, total, h8 * w8, w8,
                                                    delta == nullptr ? 1 : 0);
@@ -629,34 +601,21 @@ int pp_k_raft_coords_f32(const float* delta, float* coords1, float* hx, int hx_C
   return PP_OK;
 }
 
-int pp_k_raft_coords_init(float* coords1, __half* flow8, __half* hx, int hx_cs, int hx_flow_co, int B, int h8, int w8,
-                          cudaStream_t st) {
+int pp_k_raft_coords(const float* delta, float* coords1, __half* flow8, __half* hx, int hx_C, int hx_flow_co, int B,
+                     int h8, int w8, cudaStream_t st) {
   const long long total = (long long)B * h8 * w8;
-  raft_coords<<<nblocks(total), TPB, 0, st>>>(nullptr, coords1, flow8, hx, hx_cs, hx_flow_co, total, h8 * w8, w8, 1);
+  raft_coords<<<nblocks(total), TPB, 0, st>>>(delta, coords1, flow8, hx, hx_C, hx_flow_co, total, h8 * w8, w8,
+                                               delta == nullptr ? 1 : 0);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
 
-int pp_k_raft_coords_update(const float* delta, float* coords1, __half* flow8, __half* hx, int hx_cs, int hx_flow_co,
-                            int B, int h8, int w8, cudaStream_t st) {
-  const long long total = (long long)B * h8 * w8;
-  raft_coords<<<nblocks(total), TPB, 0, st>>>(delta, coords1, flow8, hx, hx_cs, hx_flow_co, total, h8 * w8, w8, 0);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
-
-int pp_k_convex_upsample(const float* coords1, const __half* mask, float* out_nchw, int B, int h8, int w8,
-                         cudaStream_t st) {
+template <class E>
+int pp_k_convex_upsample(const float* coords1, const E* mask, float* out_nchw, int B, int h8, int w8, cudaStream_t st) {
   const long long total = (long long)B * 64 * h8 * w8;
-  convex_upsample<__half><<<nblocks(total), TPB, 0, st>>>(coords1, mask, out_nchw, B, h8, w8);
+  convex_upsample<E><<<nblocks(total), TPB, 0, st>>>(coords1, mask, out_nchw, B, h8, w8);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }
-
-int pp_k_convex_upsample_f32(const float* coords1, const float* mask, float* out_nchw, int B, int h8, int w8,
-                             cudaStream_t st) {
-  const long long total = (long long)B * 64 * h8 * w8;
-  convex_upsample<float><<<nblocks(total), TPB, 0, st>>>(coords1, mask, out_nchw, B, h8, w8);
-  PP_CUDA_CHECK(cudaGetLastError());
-  return PP_OK;
-}
+template int pp_k_convex_upsample(const float*, const __half*, float*, int, int, int, cudaStream_t);
+template int pp_k_convex_upsample(const float*, const float*, float*, int, int, int, cudaStream_t);

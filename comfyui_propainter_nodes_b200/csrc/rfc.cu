@@ -253,67 +253,30 @@ int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows
   return PP_OK;
 }
 
-namespace {
-
-// The image-propagation kernels of one storage type: fp16 (pixel = 4 x __half, flow = __half2) or fp32 (float4 /
-// float2).  `Elem` is the element type of the arena buffers.
-struct ImgpropF16 {
-  using Elem = __half;
-  static constexpr const char* prof = "imgprop";
-  static int pack(const float* f, const float* m, Elem* d, int T, int H, int W, cudaStream_t st) {
-    return pp_k_imgprop_pack(f, m, d, T, H, W, st);
-  }
-  static int flows(const float* s, Elem* d, int n, int H, int W, cudaStream_t st) {
-    return pp_k_flow_to_nhwc2(s, d, n, H, W, st);
-  }
-  static int run(const Elem* in4, Elem* bwd, Elem* fwd, const Elem* ff, const Elem* fbk, const float* masks, int T,
-                 int H, int W, int* scratch, cudaStream_t st) {
-    return pp_k_imgprop_run(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st);
-  }
-  static int finish(const Elem* p, const float* f, const float* m, float* uf, float* um, int T, int H, int W,
-                    cudaStream_t st) {
-    return pp_k_imgprop_finish(p, f, m, uf, um, T, H, W, st);
-  }
-};
-
-struct ImgpropF32 {
-  using Elem = float;
-  static constexpr const char* prof = "imgprop_f32";
-  static int pack(const float* f, const float* m, Elem* d, int T, int H, int W, cudaStream_t st) {
-    return pp_k_imgprop_pack_f32(f, m, d, T, H, W, st);
-  }
-  static int flows(const float* s, Elem* d, int n, int H, int W, cudaStream_t st) {
-    return pp_k_flow_to_nhwc2_f32(s, d, n, H, W, st);
-  }
-  static int run(const Elem* in4, Elem* bwd, Elem* fwd, const Elem* ff, const Elem* fbk, const float* masks, int T,
-                 int H, int W, int* scratch, cudaStream_t st) {
-    return pp_k_imgprop_run_f32(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st);
-  }
-  static int finish(const Elem* p, const float* f, const float* m, float* uf, float* um, int T, int H, int W,
-                    cudaStream_t st) {
-    return pp_k_imgprop_finish_f32(p, f, m, uf, um, T, H, W, st);
-  }
-};
-
-template <class K>
-int image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f, const float* flows_b,
-                    int T, int H, int W, float* upd_frames, float* upd_masks, cudaStream_t st) {
-  using Elem = typename K::Elem;
+// Stage 3a: non-learnable image propagation (reference: propainter_inference.py:159-225 single-chunk branch,
+// model/propainter.py:118-231 with learnable=False).  One persistent kernel for the 2(T-1) serial steps.  E = float keeps
+// frames, masks and flows in fp32 (the node's fp16="disable"): the fb test, the 0.1 mask threshold and the nearest-pixel
+// pick are discrete, and an fp16-rounded flow or frame moves whole pixels, not a last bit.
+template <class E>
+int pp_stage_image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f,
+                             const float* flows_b, int T, int H, int W, float* upd_frames, float* upd_masks,
+                             cudaStream_t st) {
+  PP_REQUIRE(T >= 2, "image propagation: need at least 2 frames");
   const long long HW = (long long)H * W;
   const size_t mark0 = e.arena.mark();
-  Elem *in4, *bwd, *fwd, *ff, *fbk;
+  E *in4, *bwd, *fwd, *ff, *fbk;
   PP_TRY(pp_alloc(e, &in4, (size_t)T * HW * 4, "imgprop input"));
   PP_TRY(pp_alloc(e, &bwd, (size_t)T * HW * 4, "imgprop backward"));
   PP_TRY(pp_alloc(e, &fwd, (size_t)T * HW * 4, "imgprop forward"));
   PP_TRY(pp_alloc(e, &ff, (size_t)(T - 1) * HW * 2, "imgprop flows f"));
   PP_TRY(pp_alloc(e, &fbk, (size_t)(T - 1) * HW * 2, "imgprop flows b"));
-  PP_TRY(K::pack(frames, masks, in4, T, H, W, st));
-  PP_TRY(K::flows(flows_f, ff, T - 1, H, W, st));
-  PP_TRY(K::flows(flows_b, fbk, T - 1, H, W, st));
+  PP_TRY(pp_k_imgprop_pack(frames, masks, in4, T, H, W, st));
+  PP_TRY(pp_k_flow_to_nhwc2(flows_f, ff, T - 1, H, W, st));
+  PP_TRY(pp_k_flow_to_nhwc2(flows_b, fbk, T - 1, H, W, st));
   e.launches += 3;
   // both passes in one persistent kernel (kernels_prop.cu): bwd / fwd start as copies of the packed input, only the
   // pixels inside the hole's bounding box are touched by the 2(T-1) serial steps
-  const size_t all = (size_t)T * HW * 4 * sizeof(Elem);
+  const size_t all = (size_t)T * HW * 4 * sizeof(E);
   PP_CUDA_CHECK(cudaMemcpyAsync(bwd, in4, all, cudaMemcpyDeviceToDevice, st));
   PP_CUDA_CHECK(cudaMemcpyAsync(fwd, in4, all, cudaMemcpyDeviceToDevice, st));
   int* scratch;
@@ -321,27 +284,18 @@ int image_propagate(PPEngine& e, const float* frames, const float* masks, const 
   {
     // algorithmic bytes of the reference's 2(T-1) steps (SURVEY.md 8d: 32 B per pixel and step, fp16); the kernel
     // itself moves far less (hole pixels only + the two up-front copies)
-    const double step_bytes = 32.0 * sizeof(Elem) / sizeof(__half);
-    PPProfScope ps(e, K::prof, (double)HW * 2 * (T - 1), 0.0, (double)HW * step_bytes * 2 * (T - 1), st);
-    PP_TRY(K::run(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st));
+    const double step_bytes = 32.0 * sizeof(E) / sizeof(__half);
+    PPProfScope ps(e, sizeof(E) == 4 ? "imgprop_f32" : "imgprop", (double)HW * 2 * (T - 1), 0.0,
+                   (double)HW * step_bytes * 2 * (T - 1), st);
+    PP_TRY(pp_k_imgprop_run(in4, bwd, fwd, ff, fbk, masks, T, H, W, scratch, st));
   }
   e.launches += 4;
-  PP_TRY(K::finish(fwd, frames, masks, upd_frames, upd_masks, T, H, W, st));
+  PP_TRY(pp_k_imgprop_finish(fwd, frames, masks, upd_frames, upd_masks, T, H, W, st));
   e.launches++;
   e.arena.release(mark0);
   return PP_OK;
 }
-
-}  // namespace
-
-// Stage 3a: non-learnable image propagation (reference: propainter_inference.py:159-225 single-chunk branch,
-// model/propainter.py:118-231 with learnable=False).  One persistent kernel for the 2(T-1) serial steps.  fp32 keeps
-// frames, masks and flows in fp32 (the node's fp16="disable"): the fb test, the 0.1 mask threshold and the nearest-pixel
-// pick are discrete, and an fp16-rounded flow or frame moves whole pixels, not a last bit.
-int pp_stage_image_propagate(PPEngine& e, const float* frames, const float* masks, const float* flows_f,
-                             const float* flows_b, int T, int H, int W, float* upd_frames, float* upd_masks, bool fp32,
-                             cudaStream_t st) {
-  PP_REQUIRE(T >= 2, "image propagation: need at least 2 frames");
-  if (fp32) return image_propagate<ImgpropF32>(e, frames, masks, flows_f, flows_b, T, H, W, upd_frames, upd_masks, st);
-  return image_propagate<ImgpropF16>(e, frames, masks, flows_f, flows_b, T, H, W, upd_frames, upd_masks, st);
-}
+template int pp_stage_image_propagate<__half>(PPEngine&, const float*, const float*, const float*, const float*, int, int,
+                                              int, float*, float*, cudaStream_t);
+template int pp_stage_image_propagate<float>(PPEngine&, const float*, const float*, const float*, const float*, int, int,
+                                             int, float*, float*, cudaStream_t);

@@ -426,8 +426,7 @@ class Engine:
             pass
 
     # -- weights
-    def register_conv(self, name, w, b, groups=1, cin_map=None, macs=None):
-        packed, meta = pack_conv_weight(w, groups, cin_map)
+    def _register_packed(self, name, packed, meta, w, b, macs):
         packed = packed.to(self.device)
         bias = None if b is None else b.detach().float().contiguous().to(self.device)
         self._keep += [packed, bias]
@@ -437,17 +436,12 @@ class Engine:
                                               meta["groups"]))
         self._check(self.lib.pp_set_conv_macs(self.h, name.encode(), float(w.numel() if macs is None else macs)))
 
+    def register_conv(self, name, w, b, groups=1, cin_map=None, macs=None):
+        self._register_packed(name, *pack_conv_weight(w, groups, cin_map), w, b, macs)
+
     def register_conv_tf32(self, name, w, b, cin_map=None, macs=None):
         """Split-tf32 image of a layer (pack_conv_weight_tf32), registered as ``name + ".tf32"``."""
-        packed, meta = pack_conv_weight_tf32(w, cin_map)
-        packed = packed.to(self.device)
-        bias = None if b is None else b.detach().float().contiguous().to(self.device)
-        self._keep += [packed, bias]
-        self.conv_meta[name + ".tf32"] = meta
-        self._check(self.lib.pp_register_conv(self.h, (name + ".tf32").encode(), _ptr(packed), _ptr(bias), meta["cout_g"],
-                                              meta["cout_g_pad"], meta["bn"], meta["cin_g"], meta["kh"], meta["kw"], 1))
-        self._check(self.lib.pp_set_conv_macs(self.h, (name + ".tf32").encode(),
-                                              float(w.numel() if macs is None else macs)))
+        self._register_packed(name + ".tf32", *pack_conv_weight_tf32(w, cin_map), w, b, macs)
 
     def register_tensor(self, name, t):
         t = t.detach().float().contiguous().to(self.device)
