@@ -78,6 +78,21 @@ static int op_corr_pyramid(PPEngine& e, const void* fmap1, const void* fmap2, in
   return PP_OK;
 }
 
+// pp_flow_complete_dist / _fp32: E is the element type of the stage
+template <class E>
+static int flow_complete_dist(pp_handle h, const char* what, const float* flows_f, const float* flows_b,
+                              const float* flow_masks, int T, int H, int W, float* out_f, float* out_b, int team_first,
+                              int team_size, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(flows_f && flows_b && flow_masks && out_f && out_b, "%s: null pointer", what);
+  PP_REQUIRE(e.comm != nullptr || team_size <= 1, "%s: pp_comm_init was not called", what);
+  PP_REQUIRE(team_first >= 0 && team_size >= 1 && team_first + team_size <= e.world,
+             "%s: team [%d, %d) of %d ranks", what, team_first, team_first + team_size, e.world);
+  ArenaGuard guard(e.arena);
+  return pp_stage_flow_complete<E>(e, flows_f, flows_b, flow_masks, T, H, W, out_f, out_b, team_first, team_size,
+                                   as_stream(stream));
+}
+
 extern "C" {
 
 const char* pp_version(void) { return "propainter_b200 1 sm_90a"; }
@@ -206,19 +221,28 @@ int pp_flow_complete(pp_handle h, const float* flows_f, const float* flows_b, co
   PP_HANDLE(h);
   PP_REQUIRE(flows_f && flows_b && flow_masks && out_f && out_b, "pp_flow_complete: null pointer");
   ArenaGuard guard(e.arena);
-  return pp_stage_flow_complete(e, flows_f, flows_b, flow_masks, T, H, W, out_f, out_b, 0, 1, as_stream(stream));
+  return pp_stage_flow_complete<__half>(e, flows_f, flows_b, flow_masks, T, H, W, out_f, out_b, 0, 1,
+                                        as_stream(stream));
+}
+
+int pp_flow_complete_fp32(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T, int H,
+                          int W, float* out_f, float* out_b, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(flows_f && flows_b && flow_masks && out_f && out_b, "pp_flow_complete_fp32: null pointer");
+  ArenaGuard guard(e.arena);
+  return pp_stage_flow_complete<float>(e, flows_f, flows_b, flow_masks, T, H, W, out_f, out_b, 0, 1, as_stream(stream));
 }
 
 int pp_flow_complete_dist(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T, int H,
                           int W, float* out_f, float* out_b, int team_first, int team_size, void* stream) {
-  PP_HANDLE(h);
-  PP_REQUIRE(flows_f && flows_b && flow_masks && out_f && out_b, "pp_flow_complete_dist: null pointer");
-  PP_REQUIRE(e.comm != nullptr || team_size <= 1, "pp_flow_complete_dist: pp_comm_init was not called");
-  PP_REQUIRE(team_first >= 0 && team_size >= 1 && team_first + team_size <= e.world,
-             "pp_flow_complete_dist: team [%d, %d) of %d ranks", team_first, team_first + team_size, e.world);
-  ArenaGuard guard(e.arena);
-  return pp_stage_flow_complete(e, flows_f, flows_b, flow_masks, T, H, W, out_f, out_b, team_first, team_size,
-                                as_stream(stream));
+  return flow_complete_dist<__half>(h, "pp_flow_complete_dist", flows_f, flows_b, flow_masks, T, H, W, out_f, out_b,
+                                    team_first, team_size, stream);
+}
+
+int pp_flow_complete_dist_fp32(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
+                               int H, int W, float* out_f, float* out_b, int team_first, int team_size, void* stream) {
+  return flow_complete_dist<float>(h, "pp_flow_complete_dist_fp32", flows_f, flows_b, flow_masks, T, H, W, out_f,
+                                   out_b, team_first, team_size, stream);
 }
 
 int pp_image_propagate(pp_handle h, const float* frames, const float* masks, const float* flows_f,
@@ -462,8 +486,8 @@ int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l
 }
 
 int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, int x0_co, int x0_ch, const float* x1,
-                    int x1_C, int x1_co, int x1_ch, int N, int H, int W, int sh, int sw, int ph, int pw, int epi, int act,
-                    float slope, float scale, int act2, const float* aux0, int aux0_C, int aux0_co, float* aux1,
+                    int x1_C, int x1_co, int x1_ch, int N, int H, int W, int sh, int sw, int ph, int pw, int dh, int dw,
+                    int replicate, int epi, int act, float slope, float scale, int act2, const float* aux0, int aux0_C, int aux0_co, float* aux1,
                     int aux1_C, int aux1_co, float* out, int out_C, int out_co, int out_fp32, void* stream) {
   PP_HANDLE(h);
   PP_REQUIRE(name && x0 && out, "pp_op_conv_tf32: null pointer");
@@ -471,7 +495,7 @@ int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, in
   PPConvCall c(e, name, N, H, W);
   c.in(x0, x0_C, x0_co, x0_ch);
   if (x1 != nullptr) c.in(x1, x1_C, x1_co, x1_ch);
-  c.geom(sh, sw, ph, pw);
+  c.geom(sh, sw, ph, pw, dh, dw, replicate);
   if (out_fp32) c.out_f32(out, out_C, out_co);
   else c.out(out, out_C, out_co);
   if (epi == PP_EPI_GRU_ZR) {
@@ -483,6 +507,24 @@ int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, in
     if (aux0 != nullptr) c.residual(aux0, aux0_C, aux0_co);
   }
   return c.run(as_stream(stream));
+}
+
+int pp_op_dcn_sample_f32(pp_handle h, const float* x0, int C0, const float* x1, int C1, const float* offs, int N,
+                         int H, int W, float max_mag, float* cols, void* stream) {
+  PP_HANDLE(h);
+  const auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  PP_REQUIRE(al16(x0) && al16(x1) && al16(cols), "pp_op_dcn_sample_f32: x0, x1 and cols must be 16-byte aligned");
+  e.launches++;
+  return pp_k_dcn_sample(x0, C0, x1, C1, offs, 432, max_mag, cols, N, H, W, as_stream(stream));
+}
+
+int pp_op_upsample2x_f32(pp_handle h, const float* src, float* dst, int N, int H, int W, int C, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(src && dst, "pp_op_upsample2x_f32: null pointer");
+  PP_REQUIRE(((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0,
+             "pp_op_upsample2x_f32: src and dst must be 16-byte aligned");
+  e.launches++;
+  return pp_k_upsample2x(src, dst, N, H, W, C, as_stream(stream));
 }
 
 int pp_op_instnorm(pp_handle h, const void* x, const void* residual, void* out, int N, int HW, int C, int relu, int fp32,

@@ -165,6 +165,8 @@ int pp_raft_corr_volume(PPEngine& e, const E* fmap1, const E* fpack2, int pairs,
 // Levels 1..3 from level 0: 2x2 average pooling of each of the M query maps of h8 x w8
 template <class E>
 int pp_raft_corr_pool(PPEngine& e, E* const corr[4], long long M, int h8, int w8, cudaStream_t st);
+// Flow completion, E = float: split-tf32 activations, weights registered under "<name>.tf32" (engine.py)
+template <class E>
 int pp_stage_flow_complete(PPEngine& e, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
                            int H, int W, float* out_f, float* out_b, int team_first, int team_size, cudaStream_t st);
 // E = float: frames / masks stored as float4 and flows as float2, E = __half: 4 x fp16 / __half2

@@ -16,6 +16,8 @@ int pp_k_nchw_to_act(const float* src, __half* dst, int N, int C, int H, int W, 
 int pp_k_nchw_to_act(const float* src, float* dst, int N, int C, int H, int W, int cs, cudaStream_t st);
 int pp_k_upsample2x(const __half* src, int src_cs, int src_co, __half* dst, int dst_cs, int dst_co, int N, int H,
                     int W, int C, cudaStream_t st);
+// split-tf32 form: src [N][H][W][hi C | lo C] -> dst [N][2H][2W][hi C | lo C]
+int pp_k_upsample2x(const float* src, float* dst, int N, int H, int W, int C, cudaStream_t st);
 int pp_k_gather_blocks(void* dst, const void* src, const int* idx_dev, long long n, long long block_bytes,
                        cudaStream_t st);
 int pp_k_copy_blocks(void* dst, const int* dst_idx_dev, const void* src, const int* src_idx_dev, long long n,
@@ -75,6 +77,14 @@ int pp_k_rfc_combine(const __half* pred, int pred_cs, long long pred_tstride_pix
 int pp_k_dcn_sample(const __half* x0, int x0_cs, int x0_co, int C0, const __half* x1, int x1_cs, int x1_co, int C1,
                     const __half* offs, int offs_cs, const __half* flow, int flow_cs, int flow_co, float max_mag,
                     __half* cols, int N, int H, int W, cudaStream_t st);
+// flow completion, fp32 (split-tf32 activations): input [T][hi 4 | lo 4] (flow * (1 - m), m, 0), plain fp32 pred, and
+// the deformable sampler on split x0 / x1 (C0 + C1 = 256) with plain fp32 offsets -> split columns [pix][hi 9C | lo 9C]
+int pp_k_rfc_pack_input(const float* flows, const float* masks, float* dst, long long dst_tstride_pix, int T, int H,
+                        int W, int reverse_time, cudaStream_t st);
+int pp_k_rfc_combine(const float* pred, int pred_cs, long long pred_tstride_pix, const float* gt, const float* masks,
+                     float* out, int T, int H, int W, int reverse_time, cudaStream_t st);
+int pp_k_dcn_sample(const float* x0, int C0, const float* x1, int C1, const float* offs, int offs_cs, float max_mag,
+                    float* cols, int N, int H, int W, cudaStream_t st);
 int pp_k_featprop_cond(const __half* cur, int cur_cs, const __half* prop, int prop_cs, const __half* flow_prop,
                        const __half* flow_check, const __half* mask2, int mask_cs, __half* cond, int cond_cs, int N,
                        int H, int W, int C, cudaStream_t st);

@@ -89,6 +89,47 @@ __global__ void __launch_bounds__(256) upsample2x_ac(const __half* __restrict__ 
     }
 }
 
+// The split-tf32 form (fp32 flow completion): x = hi + lo in, tf32(y) | y - tf32(y) out.  One thread per (output pixel,
+// 4-channel vector); ATen's CPU bilinear order h0 * (w0 * a + w1 * b) + h1 * (w0 * c + w1 * d) with source index
+// (H-1)/(2H-1) * o, lambda = src - floor(src), every product and sum rounded on its own.
+__device__ __forceinline__ float4 ld_split4(const float* p, int C) {
+  const float4 h = *reinterpret_cast<const float4*>(p), l = *reinterpret_cast<const float4*>(p + C);
+  return make_float4(__fadd_rn(h.x, l.x), __fadd_rn(h.y, l.y), __fadd_rn(h.z, l.z), __fadd_rn(h.w, l.w));
+}
+__device__ __forceinline__ float lerp_rn(float a, float b, float w0, float w1) {
+  return __fadd_rn(__fmul_rn(w0, a), __fmul_rn(w1, b));
+}
+__global__ void __launch_bounds__(256) upsample2x_split(const float* __restrict__ src, float* __restrict__ dst, int H,
+                                                        int W, int C) {
+  const int OW = 2 * W, OH = 2 * H, C4 = C / 4;
+  const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (unsigned)(OW * C4)) return;
+  const int c4 = idx % (unsigned)C4, ox = idx / (unsigned)C4;
+  const int oy = blockIdx.y, n = blockIdx.z;
+  const float sy = (float)(H - 1) / (float)(OH - 1), sx = (float)(W - 1) / (float)(OW - 1);
+  const float fy = __fmul_rn(sy, (float)oy), fx = __fmul_rn(sx, (float)ox);
+  const int y0 = (int)fy, x0 = (int)fx;
+  const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
+  const float h1 = fminf(fmaxf(__fsub_rn(fy, (float)y0), 0.f), 1.f), w1 = fminf(fmaxf(__fsub_rn(fx, (float)x0), 0.f), 1.f);
+  const float h0 = __fsub_rn(1.f, h1), w0 = __fsub_rn(1.f, w1);
+  const float* base = src + (long long)n * H * W * 2 * C + 4 * c4;
+  const float4 a = ld_split4(base + (long long)(y0 * W + x0) * 2 * C, C);
+  const float4 b = ld_split4(base + (long long)(y0 * W + x1) * 2 * C, C);
+  const float4 c = ld_split4(base + (long long)(y1 * W + x0) * 2 * C, C);
+  const float4 d = ld_split4(base + (long long)(y1 * W + x1) * 2 * C, C);
+  const float r[4] = {
+      lerp_rn(lerp_rn(a.x, b.x, w0, w1), lerp_rn(c.x, d.x, w0, w1), h0, h1),
+      lerp_rn(lerp_rn(a.y, b.y, w0, w1), lerp_rn(c.y, d.y, w0, w1), h0, h1),
+      lerp_rn(lerp_rn(a.z, b.z, w0, w1), lerp_rn(c.z, d.z, w0, w1), h0, h1),
+      lerp_rn(lerp_rn(a.w, b.w, w0, w1), lerp_rn(c.w, d.w, w0, w1), h0, h1)};
+  float hi[4], lo[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) { hi[e] = ppx::tf32_rna(r[e]); lo[e] = __fsub_rn(r[e], hi[e]); }
+  float* dp = dst + ((long long)n * OH * OW + (long long)oy * OW + ox) * 2 * C + 4 * c4;
+  *reinterpret_cast<float4*>(dp) = make_float4(hi[0], hi[1], hi[2], hi[3]);
+  *reinterpret_cast<float4*>(dp + C) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+}
+
 // dst block j <- src block idx[j]; blocks are `block16` 16-byte units (frame-sized gathers for window batching)
 __global__ void gather_blocks(uint4* __restrict__ dst, const uint4* __restrict__ src, const int* __restrict__ idx,
                               long long n, long long block16) {
@@ -127,6 +168,16 @@ int pp_k_upsample2x(const __half* src, int src_cs, int src_co, __half* dst, int 
   PP_REQUIRE(H <= 65535 && N <= 65535, "upsample2x: %d rows / %d images exceed the grid limits", H, N);
   const dim3 grid(pp_ceil_div(W * (C / 8), 256), H, N);
   upsample2x_ac<<<grid, 256, 0, st>>>(src, src_cs, src_co, dst, dst_cs, dst_co, H, W, C / 8);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+int pp_k_upsample2x(const float* src, float* dst, int N, int H, int W, int C, cudaStream_t st) {
+  PP_REQUIRE(C % 4 == 0 && H >= 1 && W >= 1, "upsample2x (split): C=%d must be a multiple of 4", C);
+  if ((long long)N * H * W == 0) return PP_OK;
+  PP_REQUIRE(2 * H <= 65535 && N <= 65535, "upsample2x: %d rows / %d images exceed the grid limits", 2 * H, N);
+  const dim3 grid(pp_ceil_div(2 * W * (C / 4), 256), 2 * H, N);
+  upsample2x_split<<<grid, 256, 0, st>>>(src, dst, H, W, C);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }

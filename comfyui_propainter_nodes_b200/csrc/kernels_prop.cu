@@ -395,6 +395,25 @@ __global__ void rfc_pack_input(const float* __restrict__ flows, const float* __r
   dst[t * dst_tstride + p] = o;
 }
 
+// The fp32 form (the node's fp16="disable"): the same four channels as a split-tf32 pixel [hi 4 | lo 4]
+// (conv_igemm.cuh), the products rounded as torch's fp32 flows * (1 - masks) does.
+__global__ void rfc_pack_input_f32(const float* __restrict__ flows, const float* __restrict__ masks,
+                                   float4* __restrict__ dst, int T, long long HW, int reverse, long long dst_tstride) {
+  long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (idx >= (long long)T * HW) return;
+  const long long t = idx / HW, p = idx - t * HW;
+  const long long ts = reverse ? (T - 1 - t) : t;
+  const float m = masks[ts * HW + p];
+  const float k = __fsub_rn(1.f, m);
+  const float v[4] = {__fmul_rn(flows[(ts * 2) * HW + p], k), __fmul_rn(flows[(ts * 2 + 1) * HW + p], k), m, 0.f};
+  float hi[4], lo[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) { hi[c] = ppx::tf32_rna(v[c]); lo[c] = __fsub_rn(v[c], hi[c]); }
+  float4* d = dst + (t * dst_tstride + p) * 2;
+  d[0] = make_float4(hi[0], hi[1], hi[2], hi[3]);
+  d[1] = make_float4(lo[0], lo[1], lo[2], lo[3]);
+}
+
 // combine_flow (recurrent_flow_completion.py:389-400): out = pred*m + gt*(1-m), un-reversing time.
 __global__ void rfc_combine(const __half* __restrict__ pred, int pred_cs, const float* __restrict__ gt,
                             const float* __restrict__ masks, float* __restrict__ out, int T, long long HW,
@@ -407,6 +426,24 @@ __global__ void rfc_combine(const __half* __restrict__ pred, int pred_cs, const 
   const float m = masks[idx], k = 1.f - m;
   out[(t * 2) * HW + p] = __half2float(pr[0]) * m + gt[(t * 2) * HW + p] * k;
   out[(t * 2 + 1) * HW + p] = __half2float(pr[1]) * m + gt[(t * 2 + 1) * HW + p] * k;
+}
+
+// The fp32 form: plain fp32 pred [pix][pred_cs], torch's fp32 rounding (no contraction), so that outside the hole
+// (m = 0) the result is the input flow itself.
+__global__ void rfc_combine_f32(const float* __restrict__ pred, int pred_cs, const float* __restrict__ gt,
+                                const float* __restrict__ masks, float* __restrict__ out, int T, long long HW,
+                                int reverse, long long pred_tstride) {
+  long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (idx >= (long long)T * HW) return;
+  const long long t = idx / HW, p = idx - t * HW;
+  const long long ts = reverse ? (T - 1 - t) : t;
+  const float* pr = pred + (ts * pred_tstride + p) * pred_cs;
+  const float m = masks[idx], k = __fsub_rn(1.f, m);
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    const long long o = (t * 2 + c) * HW + p;
+    out[o] = __fadd_rn(__fmul_rn(pr[c], m), __fmul_rn(gt[o], k));
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -424,6 +461,74 @@ __global__ void dcn_sample(const PPDcnArgs a) {
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (unsigned)(a.H * a.W * 144)) return;
   dcn_sample_item<CPG, false>(a, idx, blockIdx.y);
+}
+
+// The fp32 form of dcn_sample for flow completion (16 groups of 16 channels, C = C0 + C1 = 256): inputs are split-tf32
+// tensors [pix][hi C0 | lo C0] / [pix][hi C1 | lo C1] read as x = hi + lo (exact), offsets plain fp32, columns written
+// split [pix][hi 9C | lo 9C].  Offset 5*tanh and the sigmoid modulation use the fp32-accurate ppx forms (tanhf / __expf
+// are approximations under --use_fast_math); the bilinear weights and sums follow torchvision's CPU
+// bilinear_interpolate ((w1*v1 + w2*v2) + w3*v3) + w4*v4 with every product and sum rounded on its own.
+__global__ void dcn_sample_f32(const float* __restrict__ x0, int C0, const float* __restrict__ x1, int C1,
+                               const float* __restrict__ offs, int offs_cs, float max_mag, float* __restrict__ cols,
+                               int H, int W) {
+  constexpr int CPG = 16;
+  const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (unsigned)(H * W * 144)) return;
+  const int n = blockIdx.y, C = C0 + C1;
+  const int gk = idx % 144u, pix = idx / 144u;
+  const int g = gk / 9, k = gk - g * 9;
+  const int x = pix % (unsigned)W, y = pix / (unsigned)W;
+  const long long m = (long long)n * H * W + pix;
+  const float* o = offs + m * offs_cs;
+  const float dy = __fmul_rn(max_mag, ppx::tanh_acc(o[2 * gk]));
+  const float dx = __fmul_rn(max_mag, ppx::tanh_acc(o[2 * gk + 1]));
+  const float mod = __fdiv_rn(1.f, __fadd_rn(1.f, ppx::exp_acc(-o[288 + gk])));
+  const float py = __fadd_rn((float)(y - 1 + k / 3), dy), px = __fadd_rn((float)(x - 1 + k % 3), dx);
+  float* dhi = cols + m * (long long)(18 * C) + k * C + g * CPG;
+  float* dlo = dhi + 9 * C;
+  const bool inside = py > -1.f && py < (float)H && px > -1.f && px < (float)W;
+  const int c = g * CPG;  // channel inside cat(x0, x1)
+  const float* src;
+  int Cs;
+  if (c < C0) { src = x0 + c; Cs = C0; }
+  else { src = x1 + (c - C0); Cs = C1; }
+  src += (long long)n * H * W * 2 * Cs;
+  const float fy = floorf(py), fx = floorf(px);
+  const int yl = (int)fy, xl = (int)fx;
+  const float lh = __fsub_rn(py, fy), lw = __fsub_rn(px, fx);
+  const float hh = __fsub_rn(1.f, lh), hw = __fsub_rn(1.f, lw);
+  const float wc[4] = {__fmul_rn(hh, hw), __fmul_rn(hh, lw), __fmul_rn(lh, hw), __fmul_rn(lh, lw)};
+#pragma unroll
+  for (int v = 0; v < CPG / 4; ++v) {
+    float val[4] = {0.f, 0.f, 0.f, 0.f};
+    if (inside) {
+#pragma unroll
+      for (int corner = 0; corner < 4; ++corner) {
+        const int yy = yl + (corner >> 1), xx = xl + (corner & 1);
+        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
+          const float* s = src + ((long long)yy * W + xx) * 2 * Cs + 4 * v;
+          const float4 h = *reinterpret_cast<const float4*>(s), l = *reinterpret_cast<const float4*>(s + Cs);
+          q = make_float4(__fadd_rn(h.x, l.x), __fadd_rn(h.y, l.y), __fadd_rn(h.z, l.z), __fadd_rn(h.w, l.w));
+        }
+        const float qv[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float t = __fmul_rn(wc[corner], qv[e]);
+          val[e] = corner == 0 ? t : __fadd_rn(val[e], t);
+        }
+      }
+    }
+    float hi[4], lo[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float r = __fmul_rn(mod, val[e]);
+      hi[e] = ppx::tf32_rna(r);
+      lo[e] = __fsub_rn(r, hi[e]);
+    }
+    reinterpret_cast<float4*>(dhi)[v] = make_float4(hi[0], hi[1], hi[2], hi[3]);
+    reinterpret_cast<float4*>(dlo)[v] = make_float4(lo[0], lo[1], lo[2], lo[3]);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -646,6 +751,38 @@ int pp_k_dcn_sample(const __half* x0, int x0_cs, int x0_co, int C0, const __half
   const dim3 grid(pp_ceil_div(H * W * 144, TPB), N);
   if (C == 128) dcn_sample<8><<<grid, TPB, 0, st>>>(a);
   else dcn_sample<16><<<grid, TPB, 0, st>>>(a);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+int pp_k_rfc_pack_input(const float* flows, const float* masks, float* dst, long long dst_tstride_pix, int T, int H,
+                        int W, int reverse_time, cudaStream_t st) {
+  const long long HW = (long long)H * W;
+  if (HW * T == 0) return PP_OK;
+  rfc_pack_input_f32<<<nblocks(HW * T), TPB, 0, st>>>(flows, masks, reinterpret_cast<float4*>(dst), T, HW, reverse_time,
+                                                      dst_tstride_pix);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+int pp_k_rfc_combine(const float* pred, int pred_cs, long long pred_tstride_pix, const float* gt, const float* masks,
+                     float* out, int T, int H, int W, int reverse_time, cudaStream_t st) {
+  const long long HW = (long long)H * W;
+  if (HW * T == 0) return PP_OK;
+  rfc_combine_f32<<<nblocks(HW * T), TPB, 0, st>>>(pred, pred_cs, gt, masks, out, T, HW, reverse_time, pred_tstride_pix);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+int pp_k_dcn_sample(const float* x0, int C0, const float* x1, int C1, const float* offs, int offs_cs, float max_mag,
+                    float* cols, int N, int H, int W, cudaStream_t st) {
+  PP_REQUIRE(C0 + C1 == 256 && C0 % 16 == 0, "dcn_sample (fp32): C0=%d C1=%d must be 16-channel groups of 256", C0, C1);
+  PP_REQUIRE((C1 == 0 || x1 != nullptr) && x0 != nullptr && offs != nullptr && cols != nullptr,
+             "dcn_sample (fp32): null pointer");
+  if ((long long)N * H * W == 0) return PP_OK;
+  PP_REQUIRE(N <= 65535 && (long long)H * W * 144 < (1LL << 31), "dcn_sample: %d images of %dx%d exceed the grid limits", N, W, H);
+  const dim3 grid(pp_ceil_div(H * W * 144, TPB), N);
+  dcn_sample_f32<<<grid, TPB, 0, st>>>(x0, C0, x1, C1, offs, offs_cs, max_mag, cols, H, W);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }

@@ -42,6 +42,8 @@ _SIGNATURES = {
     "pp_raft_bidir_fp32": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP]),
     "pp_flow_complete": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
     "pp_flow_complete_dist": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _I, _I, _VP]),
+    "pp_flow_complete_fp32": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
+    "pp_flow_complete_dist_fp32": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _I, _I, _VP]),
     "pp_image_propagate": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
     "pp_image_propagate_fp32": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
     "pp_gen_begin": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
@@ -61,8 +63,10 @@ _SIGNATURES = {
     "pp_profile_dump": (_I, [_VP, ctypes.c_char_p, _SZ]),
     "pp_op_conv": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _F, _VP, _VP, _VP]),
     "pp_op_corr_lookup": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
-    "pp_op_conv_tf32": (_I, [_VP, _CP, _VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _I,
-                             _VP, _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _VP]),
+    "pp_op_conv_tf32": (_I, [_VP, _CP, _VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I,
+                             _F, _F, _I, _VP, _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _VP]),
+    "pp_op_dcn_sample_f32": (_I, [_VP, _VP, _I, _VP, _I, _VP, _I, _I, _I, _F, _VP, _VP]),
+    "pp_op_upsample2x_f32": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "pp_op_instnorm": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "pp_op_corr_pyramid": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
     "pp_op_corr_lookup_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
@@ -457,14 +461,15 @@ class Engine:
         "gen.fp.backward_1.offset.0", "gen.fp.forward_1.offset.0", "gen.fp.backward_1.backbone.0",
         "gen.fp.forward_1.backbone.0", "gen.fp.fuse.0")
 
-    # fp32 RAFT path: kernel input channels of the split images whose reference channels are not a multiple of 32
+    # fp32 RAFT and flow-completion paths: kernel input channels of the split images whose reference channels are not a multiple of 32
     # (the frames: 3 -> 4, one 16-byte vector; the correlation lookup: 324 -> 352, whole 32-channel K chunks per pass)
-    TF32_CIN_MAPS = {"raft.fnet.conv1": (3, 4), "raft.cnet.conv1": (3, 4), "raft.update.convc1": (324, 352)}
+    TF32_CIN_MAPS = {"raft.fnet.conv1": (3, 4), "raft.cnet.conv1": (3, 4), "raft.update.convc1": (324, 352),
+                     "rfc.downsample": (3, 4)}
 
     def load_weights(self, raft_sd, rfc_sd, gen_sd):
         convs, tens = build_layers(raft_sd, rfc_sd, gen_sd)
         for name, (w, b, groups, cin_map, macs) in convs.items():
-            if name.startswith("raft."):
+            if name.startswith(("raft.", "rfc.")):
                 tm = self.TF32_CIN_MAPS.get(name)
                 self.register_conv_tf32(name, w, b, None if tm is None else _pad_map(*tm), macs)
             if name in self.PAD64_CONVS:
@@ -496,25 +501,31 @@ class Engine:
         self._check(fn(self.h, _ptr(frames), T, H, W, int(iters), _ptr(ff), _ptr(fb), self._stream()))
         return ff, fb
 
-    def flow_complete(self, flows_f, flows_b, flow_masks):
+    def flow_complete(self, flows_f, flows_b, flow_masks, fp32: bool = False):
+        """flows [T-1,2,H,W], flow_masks [T,1,H,W] -> completed (flows_f, flows_b).  fp32=False: fp16 activations;
+        fp32=True: fp32 activations and 3xTF32 convolutions (pp_flow_complete_fp32), what the node runs for
+        fp16="disable"."""
         flows_f, flows_b, flow_masks = self._f32(flows_f), self._f32(flows_b), self._f32(flow_masks)
         T, _, H, W = flow_masks.shape
         assert flows_f.shape[0] == T - 1
         of, ob = torch.empty_like(flows_f), torch.empty_like(flows_b)
-        self._check(self.lib.pp_flow_complete(self.h, _ptr(flows_f), _ptr(flows_b), _ptr(flow_masks), T, H, W, _ptr(of),
-                                              _ptr(ob), self._stream()))
+        fn = self.lib.pp_flow_complete_fp32 if fp32 else self.lib.pp_flow_complete
+        self._check(fn(self.h, _ptr(flows_f), _ptr(flows_b), _ptr(flow_masks), T, H, W, _ptr(of), _ptr(ob),
+                       self._stream()))
         return of, ob
 
-    def flow_complete_dist(self, flows_f, flows_b, flow_masks, team_first: int, team_size: int, out=None):
+    def flow_complete_dist(self, flows_f, flows_b, flow_masks, team_first: int, team_size: int, out=None,
+                           fp32: bool = False):
         """Collective flow completion of one chunk by the ranks [team_first, team_first + team_size) (see
-        pp_flow_complete_dist); every team member gets the full completed flows."""
+        pp_flow_complete_dist); every team member gets the full completed flows.  fp32 as in flow_complete."""
         flows_f, flows_b, flow_masks = self._f32(flows_f), self._f32(flows_b), self._f32(flow_masks)
         T, _, H, W = flow_masks.shape
         assert flows_f.shape[0] == T - 1
         of, ob = out if out is not None else (torch.empty_like(flows_f), torch.empty_like(flows_b))
         assert of.is_contiguous() and ob.is_contiguous() and of.dtype == torch.float32
-        self._check(self.lib.pp_flow_complete_dist(self.h, _ptr(flows_f), _ptr(flows_b), _ptr(flow_masks), T, H, W,
-                                                   _ptr(of), _ptr(ob), int(team_first), int(team_size), self._stream()))
+        fn = self.lib.pp_flow_complete_dist_fp32 if fp32 else self.lib.pp_flow_complete_dist
+        self._check(fn(self.h, _ptr(flows_f), _ptr(flows_b), _ptr(flow_masks), T, H, W, _ptr(of), _ptr(ob),
+                       int(team_first), int(team_size), self._stream()))
         return of, ob
 
     def image_propagate(self, frames, masks, flows_f, flows_b, fp32: bool = False):
@@ -763,10 +774,12 @@ class Engine:
     EPI_STD, EPI_GRU_ZR, EPI_GRU_H = range(3)
 
     def op_conv_tf32(self, name, inputs, out, out_co=0, stride=(1, 1), pad=(0, 0), act=ACT_NONE, slope=0.0, scale=1.0,
-                     act2=ACT_NONE, residual=None, gru_zr=None, gru_h=None, out_fp32=False):
+                     act2=ACT_NONE, residual=None, gru_zr=None, gru_h=None, out_fp32=False, dilation=(1, 1),
+                     replicate=False):
         """One split-tf32 convolution (weights from register_conv_tf32) on split tensors [N,H,W,2C] float32 (split_tf32:
         hi channels, then lo).  inputs: one or two (tensor, first channel, channels); out: split tensor written at channel
-        out_co, or with out_fp32 a plain [N,OH,OW,C] float32 tensor.  Epilogue: act / slope / scale / act2 and an optional
+        out_co, or with out_fp32 a plain [N,OH,OW,C] float32 tensor; padding is zeros or, with replicate, the edge
+        pixels.  Epilogue: act / slope / scale / act2 and an optional
         residual (tensor, co); or gru_zr = (h, h_co, rh, rh_co) (z -> out, r * h -> rh); or gru_h = (h, h_co, z, z_co)."""
         N, H, W = inputs[0][0].shape[:3]
         (x0, c0, n0), (x1, c1, n1) = inputs[0], (inputs[1] if len(inputs) > 1 else (None, 0, 0))
@@ -780,8 +793,26 @@ class Engine:
             epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_H, gru_h
         self._check(self.lib.pp_op_conv_tf32(
             self.h, (name + ".tf32").encode(), _ptr(x0), C(x0), c0, n0, _ptr(x1), C(x1), c1, n1, N, H, W, stride[0],
-            stride[1], pad[0], pad[1], epi, act, float(slope), float(scale), act2, _ptr(a0), C(a0), a0_co, _ptr(a1), C(a1),
+            stride[1], pad[0], pad[1], dilation[0], dilation[1], int(replicate), epi, act, float(slope), float(scale), act2, _ptr(a0), C(a0), a0_co, _ptr(a1), C(a1),
             a1_co, _ptr(out), out.shape[-1] if out_fp32 else C(out), out_co, int(out_fp32), self._stream()))
+        return out
+
+    def op_dcn_sample_f32(self, x0, x1, offs, max_mag=5.0):
+        """fp32 deformable sampler of flow completion: split x0 [N,H,W,2*C0] and x1 [N,H,W,2*C1] (C0 + C1 = 256), offs
+        float32 [N,H,W,432] -> split columns [N,H,W,2*2304] (hi 2304 | lo 2304, K ordered (tap, channel)).  x1 may be
+        None when x0 holds all 256 channels."""
+        N, H, W = x0.shape[:3]
+        cols = torch.empty(N, H, W, 2 * 2304, device=self.device, dtype=torch.float32)
+        C1 = 0 if x1 is None else x1.shape[-1] // 2
+        self._check(self.lib.pp_op_dcn_sample_f32(self.h, _ptr(x0), x0.shape[-1] // 2, _ptr(x1), C1, _ptr(offs), N, H,
+                                                  W, float(max_mag), _ptr(cols), self._stream()))
+        return cols
+
+    def op_upsample2x_f32(self, x):
+        """bilinear x2 (align_corners=True) of a split tensor [N,H,W,2C] -> [N,2H,2W,2C]."""
+        N, H, W, C2 = x.shape
+        out = torch.empty(N, 2 * H, 2 * W, C2, device=self.device, dtype=torch.float32)
+        self._check(self.lib.pp_op_upsample2x_f32(self.h, _ptr(x), _ptr(out), N, H, W, C2 // 2, self._stream()))
         return out
 
     def op_instnorm(self, x, C, relu=False, residual=None, out=None, fp32=True):

@@ -236,10 +236,12 @@ def complete_flow_distributed(flow_model, flows_bi, flow_masks, subvideo_length,
     """Flow completion of one clip on `world` ranks (every rank holds the full inputs, every rank gets the full
     result).  The recurrence is serial in time, so what shards is (a) the independent sub-video chunks -> teams of
     ranks, (b) inside a chunk the two direction passes and the per-frame encoder / decoder (pp_flow_complete_dist).
-    Exchange: the in-team all-gathers of the C call, then one all-gather of the chunks between teams."""
+    Exchange: the in-team all-gathers of the C call, then one all-gather of the chunks between teams.  The precision
+    follows the flows' dtype as in propainter_inference.complete_flow, so the N-GPU result equals the 1-GPU one."""
     eng = flow_model.engine
     ff, fb, fm = flows_bi[0][0], flows_bi[1][0], flow_masks[0]
     dt = flows_bi[0].dtype
+    fp32 = dt == torch.float32
     L = ff.shape[0]
     if getattr(eng, "world", 1) <= 1:      # no engine communicator (CPU/gloo logic tests): every rank computes all
         from . import propainter_inference as PI
@@ -255,7 +257,7 @@ def complete_flow_distributed(flow_model, flows_bi, flow_masks, subvideo_length,
         if team < 0 or ci >= len(chunks):
             continue
         f0, f1, s, e = chunks[ci]
-        a, b = eng.flow_complete_dist(ff32[s:e], fb32[s:e], fm32[s:e + 1], team * tsize, tsize)
+        a, b = eng.flow_complete_dist(ff32[s:e], fb32[s:e], fm32[s:e + 1], team * tsize, tsize, fp32=fp32)
         of[f0:f1] = a[f0 - s:f1 - s]
         ob[f0:f1] = b[f0 - s:f1 - s]
     if n_teams > 1 or n_teams * tsize < world:

@@ -13,8 +13,10 @@ exactly where the reference calls its PyTorch modules:
 Tensors keep the reference layouts ([1,T,C,H,W]).  RAFT follows the ``fp16`` switch: "enable" runs it with fp16
 activations and fp32 accumulation, "disable" at fp32 accuracy (fp32 activations, 3xTF32 GEMMs), like the reference,
 which always runs RAFT in fp32.  Image propagation follows it too: "disable" keeps frames, masks and flows in fp32
-(pp_image_propagate_fp32), "enable" stores them in fp16.  Flow completion and the generator compute in fp16 with fp32
-accumulation in both modes (there the switch only selects the dtype of the tensors handed back).
+(pp_image_propagate_fp32), "enable" stores them in fp16.  So does flow completion: "disable" runs it at fp32 accuracy
+(pp_flow_complete_fp32: fp32 activations, 3xTF32 GEMMs, fp32 deformable sampling), "enable" with fp16 activations and
+fp32 accumulation.  The generator computes in fp16 with fp32 accumulation in both modes (there the switch only selects
+the dtype of the tensors handed back).
 """
 from __future__ import annotations
 
@@ -73,20 +75,24 @@ def compute_flow(raft_model, frames: torch.Tensor, config: ProPainterConfig):
 
 
 def complete_flow(recurrent_flow_model, flows_tuple, flow_masks: torch.Tensor, subvideo_length: int):
-    """Recurrent flow completion, chunked exactly like the reference (temporal convs see the 5-flow halo)."""
+    """Recurrent flow completion, chunked exactly like the reference (temporal convs see the 5-flow halo).
+
+    The precision follows the dtype of the flows process_inpainting hands over, as the reference's network follows
+    ``fp16``: float32 (fp16="disable") runs at fp32 accuracy, float16 with fp16 activations."""
     eng = recurrent_flow_model.engine
     ff, fb, fm = flows_tuple[0][0], flows_tuple[1][0], flow_masks[0]
     dt = flows_tuple[0].dtype
+    fp32 = dt == torch.float32
     L = ff.shape[0]
     if L <= subvideo_length:
-        of, ob = eng.flow_complete(ff, fb, fm)
+        of, ob = eng.flow_complete(ff, fb, fm, fp32=fp32)
     else:
         pad = 5
         pf, pb = [], []
         for f in range(0, L, subvideo_length):
             s, e = max(0, f - pad), min(L, f + subvideo_length + pad)
             ps, pe = f - s, e - min(L, f + subvideo_length)
-            a, b = eng.flow_complete(ff[s:e], fb[s:e], fm[s:e + 1])
+            a, b = eng.flow_complete(ff[s:e], fb[s:e], fm[s:e + 1], fp32=fp32)
             pf.append(a[ps:e - s - pe])
             pb.append(b[ps:e - s - pe])
         of, ob = torch.cat(pf, 0), torch.cat(pb, 0)

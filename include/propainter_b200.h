@@ -7,7 +7,7 @@
  *
  *   pp_raft_bidir[_fp32]   replaces  raft_model(frames, iters)                propainter_inference.py:77-93
  *                                    (RAFT_bi.forward, model/modules/flow_comp_raft.py:39-58)
- *   pp_flow_complete       replaces  forward_bidirect_flow + combine_flow     propainter_inference.py:123-150
+ *   pp_flow_complete[_fp32] replaces forward_bidirect_flow + combine_flow     propainter_inference.py:123-150
  *                                    (model/recurrent_flow_completion.py:356-400)
  *   pp_image_propagate[_fp32] replaces img_propagation + blend               propainter_inference.py:186-219
  *                                    (model/propainter.py:350-356, 118-231)
@@ -87,6 +87,16 @@ PP_API int pp_flow_complete(pp_handle h, const float* flows_f, const float* flow
  * the completed flows (whole team) leave the full result on every rank of the team.  team_size 1 = pp_flow_complete. */
 PP_API int pp_flow_complete_dist(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
                                  int H, int W, float* out_f, float* out_b, int team_first, int team_size, void* stream);
+/* pp_flow_complete / pp_flow_complete_dist at fp32 accuracy (the node's fp16="disable"): fp32 activations, every
+ * convolution as an error-compensated tf32 GEMM (3xTF32), an fp32 deformable sampler and bilinear upsampling, and a
+ * combine that returns the input flow unchanged outside the mask.  The propagation step runs one launch per layer, and
+ * the per-frame decoder runs in frame batches sized to the free arena (the result does not depend on the batch size).
+ * Needs the flow-completion weights also registered as split images under "<name>.tf32" (engine.py registers both). */
+PP_API int pp_flow_complete_fp32(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks, int T,
+                                 int H, int W, float* out_f, float* out_b, void* stream);
+PP_API int pp_flow_complete_dist_fp32(pp_handle h, const float* flows_f, const float* flows_b, const float* flow_masks,
+                                      int T, int H, int W, float* out_f, float* out_b, int team_first, int team_size,
+                                      void* stream);
 /* frames [T,3,H,W], masks [T,1,H,W], completed flows  ->  updated frames [T,3,H,W], updated masks [T,1,H,W]. */
 PP_API int pp_image_propagate(pp_handle h, const float* frames, const float* masks, const float* flows_f,
                        const float* flows_b, int T, int H, int W, float* updated_frames, float* updated_masks,
@@ -162,18 +172,28 @@ PP_API int pp_op_conv(pp_handle h, const char* name, const void* x_f16, int N, i
                int replicate, int act, float slope, const void* residual_f16, void* out_f16, void* stream);
 PP_API int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream);
-/* Operators of the fp32 RAFT path (pp_raft_bidir_fp32).  Split tensors are fp32 [pix][hi C | lo C] with hi = tf32(x),
+/* Operators of the fp32 RAFT and flow-completion paths (pp_raft_bidir_fp32, pp_flow_complete_fp32).  Split tensors are fp32 [pix][hi C | lo C] with hi = tf32(x),
  * lo = x - hi; `*_C` is a tensor's channel count C, `*_co` / `*_ch` count channels.
  * One split-tf32 convolution with weights registered as a split image (Engine.register_conv_tf32): input x0 channels
- * [x0_co, x0_co + x0_ch) (then x1's, when x1 is not null), stride sh x sw, zero padding ph x pw, epilogue
+ * [x0_co, x0_co + x0_ch) (then x1's, when x1 is not null), stride sh x sw, padding ph x pw (zeros, or with
+ * replicate the edge pixels), dilation dh x dw, epilogue
  * epi = 0: act2(act(acc + bias) * scale + aux0), aux0 an optional split residual;
  * epi = 1 (GRU z|r): z -> out, r * aux0 (h) -> aux1 (r*h);  epi = 2 (GRU q): (1 - z) * h + z * tanh(acc + bias) -> out
  * with h = aux0, z = aux1.  out is split, written at channel out_co, or (out_fp32) plain fp32 [pix][out_C]. */
 PP_API int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, int x0_co, int x0_ch, const float* x1,
-                           int x1_C, int x1_co, int x1_ch, int N, int H, int W, int sh, int sw, int ph, int pw, int epi,
-                           int act, float slope, float scale, int act2, const float* aux0, int aux0_C, int aux0_co,
+                           int x1_C, int x1_co, int x1_ch, int N, int H, int W, int sh, int sw, int ph, int pw, int dh,
+                           int dw, int replicate, int epi, int act, float slope, float scale, int act2, const float* aux0, int aux0_C, int aux0_co,
                            float* aux1, int aux1_C, int aux1_co, float* out, int out_C, int out_co, int out_fp32,
                            void* stream);
+/* Modulated deformable sampling of pp_flow_complete_fp32 (3x3, pad 1, 16 offset groups): split inputs x0 [pix][hi C0 |
+ * lo C0] and x1 [pix][hi C1 | lo C1] (C0 + C1 = 256, images of H x W), offs plain fp32 [pix][432] (raw offset-head output:
+ * offsets max_mag * tanh, modulation sigmoid) -> split columns cols [pix][hi 2304 | lo 2304], K ordered (tap, channel).
+ * x0, x1 and cols 16-byte aligned; x1 may be NULL when C1 = 0. */
+PP_API int pp_op_dcn_sample_f32(pp_handle h, const float* x0, int C0, const float* x1, int C1, const float* offs, int N,
+                                int H, int W, float max_mag, float* cols, void* stream);
+/* Bilinear x2 upsampling (align_corners=True) of split tensors: src [N][H][W][hi C | lo C] -> dst [N][2H][2W][hi C | lo C]
+ * (16-byte aligned, C a multiple of 4). */
+PP_API int pp_op_upsample2x_f32(pp_handle h, const float* src, float* dst, int N, int H, int W, int C, void* stream);
 /* InstanceNorm2d (eps 1e-5, no affine) of N images [HW][C] (+relu) (then relu(residual + .)): fp16 [pix][C] or, with
  * fp32, split tensors.  out may be x. */
 PP_API int pp_op_instnorm(pp_handle h, const void* x, const void* residual, void* out, int N, int HW, int C, int relu,
