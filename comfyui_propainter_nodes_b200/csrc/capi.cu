@@ -476,6 +476,31 @@ int pp_op_conv(pp_handle h, const char* name, const void* x_f16, int N, int H, i
   return c.run(as_stream(stream));
 }
 
+int pp_op_conv_ex(pp_handle h, const char* name, const void* x_f16, int x_C, int x_co, int N, int H, int W, int ph,
+                  int pw, int epi, int act, float slope, float scale, int act2, const void* aux0_f16, int aux0_C,
+                  int aux0_co, void* aux1_f16, int aux1_C, int aux1_co, void* out_f16, int out_C, int out_co, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(name && x_f16 && out_f16, "pp_op_conv_ex: null pointer");
+  PP_REQUIRE(epi == PP_EPI_STD || (aux0_f16 && aux1_f16), "pp_op_conv_ex: the GRU epilogues need aux0 and aux1");
+  const PPPackedConv* w = nullptr;
+  PP_TRY(pp_get_conv(e, name, &w));
+  PPConvCall c(e, name, N, H, W);
+  c.in(static_cast<const __half*>(x_f16), x_C, x_co, w->cin_g, w->groups > 1 ? w->cin_g : 0)
+      .geom(1, 1, ph, pw)
+      .out(static_cast<__half*>(out_f16), out_C, out_co, w->groups > 1 ? w->cout_g : 0);
+  const __half* a0 = static_cast<const __half*>(aux0_f16);
+  __half* a1 = static_cast<__half*>(aux1_f16);
+  if (epi == PP_EPI_GRU_ZR) {
+    c.gru_zr(a0, aux0_C, aux0_co, a1, aux1_C, aux1_co);
+  } else if (epi == PP_EPI_GRU_H) {
+    c.gru_h(a0, aux0_C, aux0_co, a1, aux1_C, aux1_co);
+  } else {
+    c.act(act, slope, scale, act2);
+    if (a0 != nullptr) c.residual(a0, aux0_C, aux0_co);
+  }
+  return c.run(as_stream(stream));
+}
+
 int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream) {
   PP_HANDLE(h);

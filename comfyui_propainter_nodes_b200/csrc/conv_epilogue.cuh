@@ -66,8 +66,9 @@ __device__ __forceinline__ void store16(__half* dst, int nvalid, bool vec, const
 
 // `raw`: 16 fp32 accumulators (tile columns ng0-n0 .. +15) of output pixel `mrow` (flattened N*OH*OW index),
 // group g, first channel ng0 (within the group; ng0 < Cout_g).  `epi`/`vec` are launch-uniform.
-// The PP_EPI_STD branch's operation order is repeated per value by conv_gemm.cu's fragment epilogue (gemm_epi4); keep
-// the two in step, the flat layers' results do not depend on which kernel ran them.
+// The PP_EPI_STD branch's operation order is repeated per value by std_epi4 (the fragment epilogues of conv_gemm.cu and
+// conv_halo.cu), the GRU branches by conv_halo.cu's halo_frag_epilogue; keep them in step, a layer's results do not
+// depend on which kernel or epilogue path ran it.
 __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uint32_t (&raw)[16], long long mrow, int g,
                                                 int ng0, int epi, bool vec) {
     const int nvalid = min(16, p.Cout_g - ng0);
@@ -138,6 +139,27 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
       for (int i = 0; i < 16; ++i) v[i] = (1.f - z[i]) * h[i] + z[i] * v[i];
       store16(reinterpret_cast<__half*>(p.out) + mrow * p.out_cstride + p.out_coff + ng0, nvalid, vec, v);
     }
+}
+
+// 4 accumulators of one fragment column pair (rows r and r + 8, columns c, c + 1) through the PP_EPI_STD epilogue, in
+// conv_epilogue16's operation order.  ACT1: p.act1 (dispatched once per tile, so the loop over the fragments has no
+// indirect branch); act2 is applied when set.  Used by the fragment epilogues of conv_gemm.cu and conv_halo.cu.
+template <int ACT1>
+__device__ __forceinline__ void std_epi4(float (&v)[4], bool has_bias, const float2& bias, float scale, bool has_res,
+                                          const float (&res)[4], int act2, float slope) {
+  if (has_bias) {
+    v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
+  }
+  act16_t<ACT1>(v, slope);
+  if (scale != 1.f) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] *= scale;
+  }
+  if (has_res) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] += res[i];
+  }
+  if (act2 != PP_ACT_NONE) act16(v, act2, slope);
 }
 
 // ---- split-tf32 form (PPConvParams::split): fp32 [hi | lo] operands, see conv_igemm.cuh

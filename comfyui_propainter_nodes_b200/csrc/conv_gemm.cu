@@ -63,27 +63,6 @@ __device__ __forceinline__ Smem gemm_smem() {
   return m;
 }
 
-// 4 accumulators of one fragment column pair (rows r and r + 8, columns c, c + 1) through the PP_EPI_STD epilogue, in
-// conv_epilogue16's operation order.  ACT1: p.act1 (dispatched once per tile, so the loop over the fragments has no
-// indirect branch); act2 is PP_ACT_NONE on every flat layer but is still applied when set.
-template <int ACT1>
-__device__ __forceinline__ void gemm_epi4(float (&v)[4], bool has_bias, const float2& bias, float scale, bool has_res,
-                                          const float (&res)[4], int act2, float slope) {
-  if (has_bias) {
-    v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
-  }
-  ppconv::act16_t<ACT1>(v, slope);
-  if (scale != 1.f) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] *= scale;
-  }
-  if (has_res) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] += res[i];
-  }
-  if (act2 != PP_ACT_NONE) ppconv::act16(v, act2, slope);
-}
-
 // The fragment epilogue of one warpgroup into its rows of the staging tile `so`.  Every column of the tile is written
 // (the staging tile has room for all of them; columns past Cout_g are never stored), so the loop is straight-line code
 // whose shared-memory loads and stores the compiler can batch.
@@ -114,7 +93,7 @@ __device__ __forceinline__ void gemm_epilogue(const PPConvParams& p, const float
         const float2 r0 = __half22float2(*lo), r1 = __half22float2(*hi);
         res[0] = r0.x; res[1] = r0.y; res[2] = r1.x; res[3] = r1.y;
       }
-      gemm_epi4<ACT1>(v, has_bias, bias, scale, has_res, res, act2, slope);
+      ppconv::std_epi4<ACT1>(v, has_bias, bias, scale, has_res, res, act2, slope);
       *lo = __floats2half2_rn(v[0], v[1]);
       *hi = __floats2half2_rn(v[2], v[3]);
     }

@@ -18,6 +18,13 @@
 // then the fused epilogue of conv_epilogue.cuh -> global), warp 8 patch producer (TMA), warp 9 weight producer (bulk
 // copy).  MT == 1: warpgroup w owns pixel rows 64w..64w+63 of the sub-tile; MT == 2: warpgroup w owns sub-tile w.
 //
+// Epilogue.  conv_halo_kernel runs it on the wgmma fragments where the layer's output can be TMA-stored (fp16, 16-byte
+// aligned; halo_tma_configure): the tile's bias columns are copied to shared memory once, act1 is a compile-time case,
+// the residual / GRU h / GRU z operands are TMA-loaded into shared memory while the tile's last wgmmas run, results go
+// as fp16 into a swizzled staging tile that one thread per warpgroup TMA-stores, and the stores drain under the next
+// tile's main loop.  Every other layer, and the other two kernels, copy the accumulators through an fp32 staging tile 32
+// columns at a time into conv_epilogue16 (drain_acc), which loads its operands and stores per thread.
+//
 // conv_halo_tf32_kernel is the split-tf32 form (PPConvParams::split, see conv_igemm.cuh): the byte geometry is the same
 // (a 128-byte swizzled K-chunk row holds 32 fp32 channels, each chunk is 4 wgmmas m64nNk8 with the same 32-byte
 // descriptor step), so the tap views, rings and producers are shared; only the MMA instruction and the epilogue differ.
@@ -40,8 +47,9 @@ constexpr int MAX_SA = 4, MAX_SB = 8;
 // stages; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the barrier block come on top (see
 // HaloSmem)
 constexpr int SMEM_BUDGET = 186 * 1024;
+constexpr int SMEM_MAX = 227 * 1024;   // dynamic shared memory of one CTA on sm_90
 
-struct HaloParams {
+struct HaloLayer {
   PPConvParams c;
   CUtensorMap tmap[PP_MAX_SEGS];
   int MT;            // sub-tiles (128 pixels each) per CTA tile
@@ -57,10 +65,21 @@ struct HaloParams {
   int debug;         // bit 0: skip the epilogue math/stores (PP_CONV_NOEPI=1, mainloop-only timing experiments)
 };
 
+// A launch of conv_halo_kernel / conv_halo_tf32_kernel: the layer, and the tensor maps of the fp16 kernel's TMA-store
+// epilogue (conv_prog_kernel's layers are HaloLayers: they keep the drain epilogue).
+struct HaloParams : HaloLayer {
+  int tma_out;       // 1: fragment epilogue + TMA stores (halo_tma_configure); 0: the fp32 staging drain of drain_acc
+  CUtensorMap tm_out;    // out + out_coff (GRU_ZR: the z half), boxes of halo_panel_width(BN) channels x one
+                         // warpgroup's pixels
+  CUtensorMap tm_out2;   // GRU_ZR: out2 + out2_coff (r * h)
+  CUtensorMap tm_aux0;   // the residual (STD) or h (GRU), loaded into the staging tile
+  CUtensorMap tm_aux1;   // GRU_H: z, loaded one panel at a time into the z buffer
+};
+
 struct TileCoord {
   int n_idx, tx, ty, img, g;
 };
-__device__ __forceinline__ TileCoord decode_tile(const HaloParams& h, int tile) {
+__device__ __forceinline__ TileCoord decode_tile(const HaloLayer& h, int tile) {
   TileCoord t;
   t.n_idx = tile % h.n_tiles;
   int r = tile / h.n_tiles;
@@ -71,7 +90,7 @@ __device__ __forceinline__ TileCoord decode_tile(const HaloParams& h, int tile) 
   return t;
 }
 
-__host__ __device__ inline int halo_total_tiles(const HaloParams& h) {
+__host__ __device__ inline int halo_total_tiles(const HaloLayer& h) {
   return h.n_tiles * h.tiles_x * h.tiles_y * h.n_img * h.c.groups;   // < 2^31, checked by halo_configure
 }
 
@@ -81,8 +100,9 @@ struct Ring {
   uint32_t ph;
 };
 
-// Shared-memory carve-up of both halo kernels, from the 1024-byte aligned base:
+// Shared-memory carve-up of the halo kernels, from the 1024-byte aligned base:
 //   SA patch stages | SB weight stages | barrier block (1 KB) | 2 accumulator staging tiles
+// (conv_halo_kernel's TMA epilogue puts its own region in place of the staging tiles, see halo_tma_region_bytes)
 // The launchers call it with base == nullptr and read only `bytes`.
 struct HaloSmem {
   uint8_t* a;                  // patch stages (TMA, 128B swizzle: 1024-byte aligned)
@@ -110,7 +130,7 @@ __host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage
   return m;
 }
 
-// Most filter taps whose [BN x 64] weight tiles share one 16 KB weight stage (HaloParams::tps never exceeds it).
+// Most filter taps whose [BN x 64] weight tiles share one 16 KB weight stage (HaloLayer::tps never exceeds it).
 __host__ __device__ constexpr int halo_max_tps(int bn) { return 128 / bn > 1 ? 128 / bn : 1; }
 
 // One filter tap: 4 k-steps of 16 channels for each m64 block, then the descriptors move on to the next tap.
@@ -159,8 +179,55 @@ __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2],
 // its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
 // NT: see halo_tap_group.  TF32: the split-tf32 form.  PROG (conv_prog_kernel): the layer has the plain epilogue
 // (PP_EPI_STD), so the GRU epilogues are not compiled in.
+// The main loop of halo_tile into acc, for conv_halo_kernel's TMA epilogue: `before_wait` runs once the tile's last
+// commit group is issued, before the wait for it (the epilogue issues its operand loads there).  halo_tile keeps its
+// own copy of the loop so that the kernels on the drain epilogue (conv_prog_kernel, conv_halo_tf32_kernel) compile
+// to the same code as before.
+template <int BN, int MB, int NT, class BeforeWait>
+__device__ __forceinline__ void halo_mainloop(const HaloLayer& h, const HaloSmem& m, Ring& ra, Ring& rb, int wg,
+                                              float (&acc)[MB][BN / 2], BeforeWait&& before_wait) {
+  using namespace ppx;
+  const PPConvParams& p = h.c;
+  const int taps = p.kh * p.kw;
+  const uint32_t sbo = h.flat ? 1024u : (uint32_t)h.BW * 128;
+  const uint32_t step_x = (uint32_t)p.dw * 8;                                 // next tap in the row (16-byte units)
+  const uint32_t step_row = (uint32_t)(p.dh * h.BW - (p.kw - 1) * p.dw) * 8;  // last tap of a row -> next row
+  const uint32_t tap16 = (uint32_t)p.BN * 8;                                  // next tap's weight tile in the stage
+  const int kw = p.kw;
+  uint32_t aoff[MB];
+#pragma unroll
+  for (int b = 0; b < MB; ++b) aoff[b] = MB == 2 ? wg * h.sub_bytes + b * 8 * sbo : wg * 8 * sbo;
+  uint32_t accum = 0;
+  int pend_a = -1, pend_b = -1;
+  for (int c = 0; c < h.chunks; ++c) {
+    mbar_wait(&m.a_full[ra.s], ra.ph);
+    uint64_t adesc[MB];
+#pragma unroll
+    for (int b = 0; b < MB; ++b) adesc[b] = gmma_desc_sw128_kmajor(smem_u32(m.a + ra.s * m.a_stage_bytes) + aoff[b], sbo);
+    int kx = 0;
+    for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
+      mbar_wait(&m.b_full[rb.s], rb.ph);
+      const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(m.b + rb.s * m.b_stage_bytes));
+      halo_tap_group<BN, MB, NT, false>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+      wgmma_wait<1>();
+      if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
+      if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
+      pend_b = rb.s;
+      pend_a = tap0 + h.tps >= taps ? ra.s : -1;
+      if (++rb.s == m.SB) { rb.s = 0; rb.ph ^= 1; }
+    }
+    if (++ra.s == m.SA) { ra.s = 0; ra.ph ^= 1; }
+  }
+  before_wait();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int b = 0; b < MB; ++b) wgmma_fence_acc(acc[b]);
+  if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
+  if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
+}
+
 template <int BN, int MB, int NT, bool TF32 = false, bool PROG = false>
-__device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
+__device__ __forceinline__ void halo_tile(const HaloLayer& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
                                           int wg, int t128) {
   using namespace ppx;
   const PPConvParams& p = h.c;
@@ -227,6 +294,190 @@ __device__ __forceinline__ void halo_tile(const HaloParams& h, int tile, const H
   }
 }
 
+// ---- conv_halo_kernel's TMA epilogue (HaloParams::tma_out)
+// After the barrier block, in place of the drain's fp32 staging tiles:
+//   fp16 staging tile | the tile's bias columns | GRU_H: one z panel per warpgroup
+// The staging tile holds, per consumer warpgroup, BN / pw panels of [64 MT pixels][pw channels], each swizzled like the
+// TMA box that stores it (128B / 64B / 32B swizzle for 64 / 32 / 16 channels).  A warpgroup's pixels are its 8 x 16
+// (MT = 2) or 8 x 8 (MT = 1) block of the tile, or its run of consecutive pixels in flat mode, in box order, so row r of
+// a panel is accumulator row r of the warpgroup.
+__host__ __device__ constexpr int halo_panel_width(int bn) { return bn % 64 == 0 ? 64 : bn % 32 == 0 ? 32 : 16; }
+__host__ __device__ constexpr int halo_out_stage_bytes(int mt, int bn) { return 2 * 64 * mt * bn * 2; }
+__host__ __device__ constexpr int halo_out_bias_bytes(int bn) { return (2 * bn * 4 + 1023) / 1024 * 1024; }
+__host__ __device__ constexpr int halo_out_z_bytes(int mt, int bn) { return 2 * 64 * mt * halo_panel_width(bn) * 2; }
+__host__ __device__ constexpr int halo_tma_region_bytes(int mt, int bn, bool gru_h) {
+  return halo_out_stage_bytes(mt, bn) + halo_out_bias_bytes(bn) + (gru_h ? halo_out_z_bytes(mt, bn) : 0);
+}
+// barriers of the operand loads, one per consumer warpgroup, behind HaloSmem::spare
+__device__ __forceinline__ uint64_t* halo_out_bar(const HaloSmem& m, int wg) { return m.spare + 1 + wg; }
+
+// Byte offset of (row r, channel c % PW) within a panel: rows of PW * 2 bytes, the box swizzle XORs the 16-byte unit
+// index with address bits 7.. (panels start 1024-byte aligned, so panel-relative bits are absolute ones)
+template <int PW>
+__device__ __forceinline__ uint32_t halo_stg_off(int r, int c) {
+  const uint32_t off = (uint32_t)(r * PW * 2 + (c % PW) * 2);
+  return off ^ ((off >> 3) & (uint32_t)((PW / 8 - 1) << 4));
+}
+
+// The fragment epilogue of one warpgroup into its staging tile `so` (conv_epilogue16's operation order per value).
+// STD: std_epi4, the residual read from the staging tile (TMA-loaded there) and overwritten in place.  GRU_ZR: sigmoid;
+// r tiles multiply by h (in the staging tile).  GRU_H: tanh, then (1 - z) h + z q with h in the staging tile and z in the
+// warpgroup's z panel `zb`, which holds one panel at a time: panel P of the tile reads it.
+template <int MB, int BN, int EPI, int ACT1>
+__device__ __forceinline__ void halo_frag_epilogue(const PPConvParams& p, const float (&acc)[MB][BN / 2], uint8_t* so,
+                                                   const uint8_t* zb, const float* bs, bool has_aux, bool r_tile, int P,
+                                                   int t128) {
+  constexpr int PW = halo_panel_width(BN);
+  constexpr int PANEL = 64 * MB * PW * 2;
+  const bool has_bias = p.bias != nullptr;
+  const float scale = p.scale, slope = p.slope;
+  const int act2 = p.act2;
+  // fragment of m64nNk16: register 4j + i of thread t holds row 16 * (t / 32) + (t % 32) / 4 + 8 * (i / 2), column
+  // 8j + 2 * (t % 4) + i % 2
+  const int fr = 16 * (t128 >> 5) + ((t128 & 31) >> 2), fc = 2 * (t128 & 3);
+#pragma unroll
+  for (int b = 0; b < MB; ++b) {
+    const int r = 64 * b + fr;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = 8 * j + fc;
+      if (EPI == PP_EPI_GRU_H && col / PW != P) continue;
+      // rows r and r + 8 differ above the swizzle's row bits
+      const uint32_t off = (col / PW) * PANEL + halo_stg_off<PW>(r, col);
+      __half2* lo = reinterpret_cast<__half2*>(so + off);
+      __half2* hi = reinterpret_cast<__half2*>(so + off + 8 * PW * 2);
+      const float2 bias = *reinterpret_cast<const float2*>(bs + col);
+      float v[4] = {acc[b][4 * j], acc[b][4 * j + 1], acc[b][4 * j + 2], acc[b][4 * j + 3]};
+      float a[4] = {0.f, 0.f, 0.f, 0.f};
+      if (has_aux) {
+        const float2 a0 = __half22float2(*lo), a1 = __half22float2(*hi);
+        a[0] = a0.x; a[1] = a0.y; a[2] = a1.x; a[3] = a1.y;
+      }
+      if constexpr (EPI == PP_EPI_STD) {
+        ppconv::std_epi4<ACT1>(v, has_bias, bias, scale, has_aux, a, act2, slope);
+      } else {
+        if (has_bias) {
+          v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
+        }
+        if constexpr (EPI == PP_EPI_GRU_ZR) {
+          ppconv::act16_t<PP_ACT_SIGMOID>(v, 0.f);
+          if (r_tile) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) v[i] *= a[i];
+          }
+        } else {
+          const uint32_t zoff = halo_stg_off<PW>(r, col);
+          const float2 z0 = __half22float2(*reinterpret_cast<const __half2*>(zb + zoff));
+          const float2 z1 = __half22float2(*reinterpret_cast<const __half2*>(zb + zoff + 8 * PW * 2));
+          const float z[4] = {z0.x, z0.y, z1.x, z1.y};
+          ppconv::act16_t<PP_ACT_TANH>(v, 0.f);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] = (1.f - z[i]) * a[i] + z[i] * v[i];
+        }
+      }
+      *lo = __floats2half2_rn(v[0], v[1]);
+      *hi = __floats2half2_rn(v[2], v[3]);
+    }
+  }
+}
+
+// One tile of one consumer warpgroup on the TMA path: the main loop; the operand loads of the epilogue (residual / h
+// into the staging tile, GRU_H's first z panel) issued once the last commit group is out, so they overlap its wgmmas;
+// the fragment epilogue into the staging tile; this warpgroup's TMA stores, which drain under the next tile's main
+// loop.  The staging tile is waited for (cp.async.bulk.wait_group.read) only before it is written again.  `xph`: the
+// parity of this warpgroup's operand-load barrier.
+template <int BN, int MB, int NT>
+__device__ __forceinline__ void halo_tile_tma(const HaloParams& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb,
+                                              uint32_t& xph, int wg, int t128) {
+  using namespace ppx;
+  const PPConvParams& p = h.c;
+  constexpr int PW = halo_panel_width(BN);
+  constexpr int PANEL = 64 * MB * PW * 2;
+  const TileCoord t = decode_tile(h, tile);
+  const int n0 = t.n_idx * BN;
+  const int epi = p.epi;
+  const int half_c = p.Cout_g >> 1;
+  const bool r_tile = epi == PP_EPI_GRU_ZR && n0 >= half_c;   // GRU_ZR: BN divides half_c (halo_tma_configure)
+  const bool has_aux = epi == PP_EPI_STD ? p.aux0 != nullptr : (epi == PP_EPI_GRU_H || r_tile);
+  const int npanel = (min(BN, p.Cout_g - n0) + PW - 1) / PW;   // panels with channels to store; TMA clips the last one
+  uint8_t* so = reinterpret_cast<uint8_t*>(m.acc_stg) + wg * (64 * MB * BN * 2);
+  float* bs = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(m.acc_stg) + halo_out_stage_bytes(MB, BN)) + wg * BN;
+  uint8_t* zb = reinterpret_cast<uint8_t*>(bs - wg * BN) + halo_out_bias_bytes(BN) + wg * PANEL;
+  uint64_t* xbar = halo_out_bar(m, wg);
+  // this warpgroup's box: pixel coordinates (flat: first pixel) and image
+  int x0, y0, img;
+  if (h.flat) {
+    x0 = MB == 2 ? (t.tx * 2 + wg) * 128 : t.tx * 128 + 64 * wg; y0 = 0; img = 0;
+  } else {
+    x0 = t.tx * (8 * MB) + (MB == 2 ? 8 * wg : 0); y0 = t.ty * 16 + (MB == 2 ? 0 : 8 * wg); img = t.img;
+  }
+  const int aux_c = r_tile ? n0 - half_c : n0;
+  const bool issuer = t128 == 0;
+  const bool skip = (h.debug & 1) != 0;
+  float acc[MB][BN / 2];
+  halo_mainloop<BN, MB, NT>(h, m, ra, rb, wg, acc, [&] {
+    if (issuer && has_aux && !skip) {
+      tma_store_wait_read<0>();   // the previous tile's stores have read the staging tile
+      const int nz = epi == PP_EPI_GRU_H ? 1 : 0;
+      mbar_arrive_expect_tx(xbar, (uint32_t)((npanel + nz) * PANEL));
+      for (int pn = 0; pn < npanel; ++pn)
+        tma_load_4d(smem_u32(so + pn * PANEL), &h.tm_aux0, aux_c + pn * PW, x0, y0, img, xbar);
+      if (nz) tma_load_4d(smem_u32(zb), &h.tm_aux1, n0, x0, y0, img, xbar);
+    }
+  });
+  if (skip) return;
+
+  // the tile's bias columns; the previous tile's readers of this copy have passed its last named barrier
+  {
+    const int c0 = 2 * t128, n = t.g * p.Cout_g + n0 + c0;
+    float2 bv = make_float2(0.f, 0.f);
+    if (p.bias != nullptr && c0 < BN) {
+      if (n0 + c0 < p.Cout_g) bv.x = __ldg(p.bias + n);
+      if (n0 + c0 + 1 < p.Cout_g) bv.y = __ldg(p.bias + n + 1);
+    }
+    if (c0 < BN) *reinterpret_cast<float2*>(bs + c0) = bv;
+  }
+  const int bar_id = 4 + wg;
+  if (issuer && !has_aux) tma_store_wait_read<0>();
+  named_bar(bar_id, 128);
+  if (has_aux) {
+    mbar_wait(xbar, xph);
+    xph ^= 1;
+  }
+  if (epi == PP_EPI_STD) {
+    switch (p.act1) {
+      case PP_ACT_RELU: halo_frag_epilogue<MB, BN, PP_EPI_STD, PP_ACT_RELU>(p, acc, so, zb, bs, has_aux, false, 0, t128); break;
+      case PP_ACT_LRELU: halo_frag_epilogue<MB, BN, PP_EPI_STD, PP_ACT_LRELU>(p, acc, so, zb, bs, has_aux, false, 0, t128); break;
+      default: halo_frag_epilogue<MB, BN, PP_EPI_STD, PP_ACT_NONE>(p, acc, so, zb, bs, has_aux, false, 0, t128); break;
+    }
+  } else if (epi == PP_EPI_GRU_ZR) {
+    halo_frag_epilogue<MB, BN, PP_EPI_GRU_ZR, PP_ACT_NONE>(p, acc, so, zb, bs, r_tile, r_tile, 0, t128);
+  } else {
+    // one z panel at a time: before the next one is loaded, every thread has read the current one
+#pragma unroll 1
+    for (int pn = 0; pn < npanel; ++pn) {
+      if (pn > 0) {
+        named_bar(bar_id, 128);
+        if (issuer) {
+          mbar_arrive_expect_tx(xbar, (uint32_t)PANEL);
+          tma_load_4d(smem_u32(zb), &h.tm_aux1, n0 + pn * PW, x0, y0, img, xbar);
+        }
+        mbar_wait(xbar, xph);
+        xph ^= 1;
+      }
+      halo_frag_epilogue<MB, BN, PP_EPI_GRU_H, PP_ACT_NONE>(p, acc, so, zb, bs, true, false, pn, t128);
+    }
+  }
+  fence_proxy_async();           // generic-proxy smem writes -> visible to the TMA stores
+  named_bar(bar_id, 128);
+  if (issuer) {
+    const CUtensorMap* tm = r_tile ? &h.tm_out2 : &h.tm_out;
+    const int c0 = r_tile ? n0 - half_c : t.g * p.out_gstep + n0;
+    for (int pn = 0; pn < npanel; ++pn) tma_store_4d(tm, smem_u32(so + pn * PANEL), c0 + pn * PW, x0, y0, img);
+    tma_store_commit();
+  }
+}
+
 // f(IntC<BN>, IntC<MT>) for the layer's runtime tile shape (MT == 2 layers have BN <= 128)
 template <class F>
 __device__ __forceinline__ void with_tile_shape(int mt, int bn, F&& f) {
@@ -244,7 +495,7 @@ __device__ __forceinline__ void halo_smem_init_barriers(const HaloSmem& m) {
 
 // Input patch producer (TMA, one elected thread): one box load per 64-channel chunk of each of this CTA's tiles of one
 // layer.  `r` runs on across the layers of a program.
-__device__ __forceinline__ void halo_produce_patches(const HaloParams& h, const HaloSmem& m, Ring& r) {
+__device__ __forceinline__ void halo_produce_patches(const HaloLayer& h, const HaloSmem& m, Ring& r) {
   using namespace ppx;
   const PPConvParams& p = h.c;
   const int total_tiles = halo_total_tiles(h);
@@ -266,7 +517,7 @@ __device__ __forceinline__ void halo_produce_patches(const HaloParams& h, const 
 
 // Weight tile producer (bulk copy, one elected thread): per chunk, the [BN x 64] tiles of the filter taps in groups of
 // h.tps per stage.  `r` runs on across the layers of a program.
-__device__ __forceinline__ void halo_produce_weights(const HaloParams& h, const HaloSmem& m, Ring& r) {
+__device__ __forceinline__ void halo_produce_weights(const HaloLayer& h, const HaloSmem& m, Ring& r) {
   using namespace ppx;
   const PPConvParams& p = h.c;
   const int total_tiles = halo_total_tiles(h);
@@ -297,7 +548,13 @@ __device__ __forceinline__ void halo_body(const HaloParams& h) {
   using namespace ppx;
   const HaloSmem m = halo_smem(dyn_smem_1024(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes);
   const int tid = threadIdx.x, warp = tid >> 5;
-  if (tid == 0) halo_smem_init_barriers(m);
+  if (tid == 0) {
+    if constexpr (!TF32) {
+      mbar_init(halo_out_bar(m, 0), 1);
+      mbar_init(halo_out_bar(m, 1), 1);
+    }
+    halo_smem_init_barriers(m);
+  }
   __syncthreads();
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -312,6 +569,18 @@ __device__ __forceinline__ void halo_body(const HaloParams& h) {
     float* stg = m.acc_stg + wg * (ppconv::STG_BYTES / 4);
     Ring ra = {0, 0}, rb = {0, 0};
     const int total_tiles = halo_total_tiles(h);
+    if constexpr (!TF32) {
+      if (h.tma_out) {
+        uint32_t xph = 0;
+        with_tile_shape(h.MT, h.c.BN, [&](auto bn, auto mb) {
+          constexpr int BN = decltype(bn)::value;
+          for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
+            halo_tile_tma<BN, decltype(mb)::value, halo_max_tps(BN)>(h, tile, m, ra, rb, xph, wg, t128);
+        });
+        if (t128 == 0) tma_store_wait<0>();   // this warpgroup's last stores are complete
+        return;
+      }
+    }
     with_tile_shape(h.MT, h.c.BN, [&](auto bn, auto mb) {
       constexpr int BN = decltype(bn)::value;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x)
@@ -381,7 +650,7 @@ struct ProgParams {
   unsigned long long* ts;                     // debug (PP_PROG_TS=1): globaltimer of CTA 0 at [layer start, layer end]
   int kind[PROG_MAX_LAYERS];
   PPDcnArgs dcn[PROG_MAX_LAYERS];
-  HaloParams layer[PROG_MAX_LAYERS];
+  HaloLayer layer[PROG_MAX_LAYERS];
 };
 
 __device__ __forceinline__ void prog_wait(const unsigned int* counter, unsigned int target) {
@@ -450,7 +719,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
           }
         }
       } else {
-        const HaloParams& h = P.layer[li];
+        const HaloLayer& h = P.layer[li];
         const int total_tiles = halo_total_tiles(h);
         // program layers are configured with MT == 1 and BN in PROG_WIDTHS (halo_configure, one_wave)
         with_prog_width(h.c.BN, [&](auto bn) {
@@ -515,11 +784,12 @@ int pp_conv_halo_eligible(const PPConvParams& p) {
 
 namespace {
 
-// The dynamic shared memory limit of the three halo kernels, raised once before the first launch.
+// The dynamic shared memory limits of the three halo kernels (conv_halo_kernel's TMA epilogue uses all an SM has),
+// raised once before the first launch.
 int halo_set_smem_limit() {
   static bool done = false;
   if (!done) {
-    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_halo_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     PP_CUDA_CHECK(cudaFuncSetAttribute(conv_prog_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     done = true;
@@ -540,10 +810,67 @@ bool halo_stages(int budget, int a_bytes, int b_bytes, int& sa, int& sb) {
   return false;
 }
 
+// h.SA / h.SB for stages in `budget` bytes (halo_stages, then a 4th patch stage where that leaves the weight ring full).
+bool halo_layer_stages(int budget, HaloLayer& h) {
+  int sa = 0, sb = 0;
+  if (!halo_stages(budget, h.a_stage_bytes, h.b_stage_bytes, sa, sb)) return false;
+  if (sa == 3 && sb == MAX_SB && (budget - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
+  h.SA = sa; h.SB = sb;
+  return true;
+}
+
+bool aligned16(const void* ptr, int cstride, int coff) {
+  return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cstride % 8 == 0 && coff % 8 == 0;
+}
+
+// conv_halo_kernel's TMA epilogue for a configured fp16 layer: its tensor maps, and the stages that fit next to the
+// staging tile.  false: the layer keeps the drain epilogue (plain fp32 output, an activation without a compiled-in
+// case, 16-byte misaligned outputs or operands, a channel count that is not a multiple of 8, grouped outputs that are
+// not packed per group, GRU_ZR tiles that straddle the z | r boundary, or stages that do not fit).
+bool halo_tma_configure(HaloParams& h) {
+  const PPConvParams& p = h.c;
+  const int bn = p.BN, pw = halo_panel_width(bn), rows = 64 * h.MT;
+  if (p.split || p.out_fp32) return false;
+  if (p.epi == PP_EPI_STD && p.act1 != PP_ACT_NONE && p.act1 != PP_ACT_RELU && p.act1 != PP_ACT_LRELU) return false;
+  if (p.epi != PP_EPI_STD && p.groups != 1) return false;
+  if (p.epi == PP_EPI_STD && p.aux0 != nullptr && p.groups != 1) return false;
+  if (p.groups > 1 && (p.out_gstep != p.Cout_g || p.Cout_g % pw != 0)) return false;
+  if (p.epi == PP_EPI_GRU_ZR && (p.Cout_g % 2 != 0 || (p.Cout_g / 2) % bn != 0)) return false;
+  if (!aligned16(p.out, p.out_cstride, p.out_coff) || (p.groups > 1 && p.out_gstep % 8 != 0)) return false;
+  // TMA stores clip the channel dimension at 16-byte granularity (measured on H100: a 126-channel map wrote channels
+  // 126 and 127), so a channel count that ends inside a 16-byte unit would overwrite its neighbours
+  if (p.Cout_g % 8 != 0) return false;
+  if (p.aux0 != nullptr && !aligned16(p.aux0, p.aux0_cstride, p.aux0_coff)) return false;
+  if (p.epi == PP_EPI_GRU_H && !aligned16(p.aux1, p.aux1_cstride, p.aux1_coff)) return false;
+  if (p.epi == PP_EPI_GRU_ZR && !aligned16(p.out2, p.out2_cstride, p.out2_coff)) return false;
+  const int region = halo_tma_region_bytes(h.MT, bn, p.epi == PP_EPI_GRU_H);
+  HaloLayer staged = h;
+  if (!halo_layer_stages(SMEM_MAX - 2048 - region, staged)) return false;
+  h.SA = staged.SA; h.SB = staged.SB;
+  // maps: (channels, x, y, image) boxes of pw x 8 x rows / 8, or (channels, pixel) boxes of pw x rows in flat mode
+  auto map = [&](CUtensorMap* m, const __half* base, int cols, int cstride) {
+    return h.flat ? pp_tmap_pixels_f16(m, base, cols, cstride, p.M_total, 1, 1, pw, rows, 1)
+                  : pp_tmap_pixels_f16(m, base, cols, cstride, p.OW, p.OH, p.N, pw, 8, rows / 8);
+  };
+  const __half* out = static_cast<const __half*>(p.out) + p.out_coff;
+  const int half_c = p.Cout_g / 2;
+  if (p.epi == PP_EPI_GRU_ZR) {
+    if (map(&h.tm_out, out, half_c, p.out_cstride) != PP_OK) return false;
+    if (map(&h.tm_out2, p.out2 + p.out2_coff, half_c, p.out2_cstride) != PP_OK) return false;
+    if (map(&h.tm_aux0, p.aux0 + p.aux0_coff, half_c, p.aux0_cstride) != PP_OK) return false;
+  } else {
+    if (map(&h.tm_out, out, (p.groups - 1) * p.out_gstep + p.Cout_g, p.out_cstride) != PP_OK) return false;
+    if (p.aux0 != nullptr && map(&h.tm_aux0, p.aux0 + p.aux0_coff, p.Cout_g, p.aux0_cstride) != PP_OK) return false;
+    if (p.epi == PP_EPI_GRU_H && map(&h.tm_aux1, p.aux1 + p.aux1_coff, p.Cout_g, p.aux1_cstride) != PP_OK) return false;
+  }
+  h.tma_out = 1;
+  return true;
+}
+
 // Tile shape, pipeline depth and tensor maps of one layer.  one_wave: the layer is one of a multi-layer program whose
 // layers are separated by grid-wide barriers -- prefer the least work per CTA (a second, partial wave doubles the
 // layer's latency) over fewer weight re-reads, among the tile widths the program kernel instantiates.
-int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
+int halo_configure(const PPConvParams& pin, HaloLayer& h, bool one_wave) {
   h.c = pin;
   PPConvParams& p = h.c;
   int num_sms = 0;
@@ -587,14 +914,10 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
   h.n_tiles = pp_ceil_div(p.Cout_g_pad, bn);
   h.chunks = pp_ceil_div(p.Cin, 64);
   h.a_stage_bytes = pp_ceil_div(h.BW * h.BH * 128, 1024) * 1024;
-  // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloParams::tps
+  // narrow N tiles: several filter taps per weight stage (<= 16 KB), see HaloLayer::tps
   h.tps = min(halo_max_tps(bn), p.kh * p.kw);
   h.b_stage_bytes = h.tps * bn * 128;
-  int sa = 0, sb = 0;
-  PP_REQUIRE(halo_stages(SMEM_BUDGET, h.a_stage_bytes, h.b_stage_bytes, sa, sb),
-             "conv_halo: patch %dx%d does not fit shared memory", h.BW, h.BH);
-  if (sa == 3 && sb == MAX_SB && (SMEM_BUDGET - 4 * h.a_stage_bytes) / h.b_stage_bytes >= MAX_SB) sa = 4;
-  h.SA = sa; h.SB = sb;
+  PP_REQUIRE(halo_layer_stages(SMEM_BUDGET, h), "conv_halo: patch %dx%d does not fit shared memory", h.BW, h.BH);
   h.debug = pp_conv_noepi();
   const long long total_tiles = count(mt, bn);
   PP_REQUIRE(total_tiles < (1LL << 31), "conv_halo: too many tiles");
@@ -605,11 +928,17 @@ int halo_configure(const PPConvParams& pin, HaloParams& h, bool one_wave) {
 
 int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   HaloParams h;
+  memset(&h, 0, sizeof(h));
   PP_TRY(halo_configure(pin, h, false));
   PP_TRY(halo_set_smem_limit());
   int num_sms = 0;
   PP_TRY(pp_num_sms(&num_sms));
-  const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes;
+  int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes;
+  if (halo_tma_configure(h)) {
+    // the TMA epilogue's region takes the place of the drain's staging tiles
+    smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes - 2 * ppconv::STG_BYTES +
+           halo_tma_region_bytes(h.MT, h.c.BN, h.c.epi == PP_EPI_GRU_H);
+  }
   return pp_conv_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms),
                         NUM_THREADS, smem, stream);
 }
@@ -648,7 +977,7 @@ int pp_prog_record_conv(const PPConvParams& p) {
   PP_REQUIRE(p.epi == PP_EPI_STD, "conv program: only the plain epilogue (bias, activations, residual) is compiled in");
   const int li = r->prog.n_layers;
   PP_TRY(halo_configure(p, r->prog.layer[li], true));
-  const HaloParams& h = r->prog.layer[li];
+  const HaloLayer& h = r->prog.layer[li];
   PP_REQUIRE(h.MT == 1 && (h.c.BN == PROG_WIDTHS[0] || h.c.BN == PROG_WIDTHS[1] || h.c.BN == PROG_WIDTHS[2]),
              "conv program: layer tile %d x %d columns is not instantiated", h.MT, h.c.BN);
   r->prog.kind[li] = PROG_CONV;
@@ -710,7 +1039,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
     ++ts_printed;
     fprintf(stderr, "[prog %d] %d layers:", ts_printed, P.n_layers);
     for (int i = 0; i < P.n_layers; ++i) {
-      const HaloParams& L = P.layer[i];
+      const HaloLayer& L = P.layer[i];
       if (P.kind[i] == PROG_CONV)
         fprintf(stderr, " | conv K=%d N=%d bn=%d mt=%d tiles=%d: %.1f us (gap %.1f)", L.c.K_total, L.c.Cout_g, L.c.BN, L.MT,
                 halo_total_tiles(L), (h[2 * i + 1] - h[2 * i]) / 1e3, i ? (h[2 * i] - h[2 * i - 1]) / 1e3 : 0.0);

@@ -358,3 +358,23 @@ int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long row
   PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled (2-D, %d x %lld, ld %d) failed (%d)", cols, rows, ld, (int)r);
   return PP_OK;
 }
+
+int pp_tmap_pixels_f16(CUtensorMap* map, const __half* base, int cols, int cstride, long long w, int h, int n, int box_c,
+                       int box_w, int box_h) {
+  EncodeTiledFn enc = encode_fn();
+  PP_REQUIRE(enc != nullptr, "conv: cuTensorMapEncodeTiled is not available");
+  const cuuint64_t pix = (cuuint64_t)cstride * 2;
+  cuuint64_t dims[4] = {(cuuint64_t)cols, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  cuuint64_t strides[3] = {pix, (cuuint64_t)w * pix, (cuuint64_t)w * h * pix};
+  cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  const CUtensorMapSwizzle swz = box_c == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : box_c == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                                                        : CU_TENSOR_MAP_SWIZZLE_32B;
+  PP_REQUIRE(box_c == 64 || box_c == 32 || box_c == 16, "conv: pixel tensor map box of %d channels", box_c);
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), dims, strides, box, es,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  PP_REQUIRE(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled (%d ch x %lld x %d x %d, cstride %d) failed (%d)", cols, w, h, n,
+             cstride, (int)r);
+  return PP_OK;
+}

@@ -90,6 +90,10 @@ bool pp_tmap_supported();
 // pixels as one dimension.  And a 2-D [rows][cols] map with row stride `ld` and 64 x box_rows boxes.
 int pp_conv_input_tmaps(const PPConvParams& p, int bw, int bh, bool flat, CUtensorMap* maps);
 int pp_tmap_2d_f16(CUtensorMap* map, const __half* base, int cols, long long rows, int ld, int box_rows);
+// A 4-D [n][h][w][cols] map of a pixel tensor with `cstride` elements per pixel (flat: w pixels, h = n = 1), boxes of
+// box_c channels (64, 32 or 16: 128B, 64B or 32B swizzle) x box_w x box_h pixels.
+int pp_tmap_pixels_f16(CUtensorMap* map, const __half* base, int cols, int cstride, long long w, int h, int n, int box_c,
+                       int box_w, int box_h);
 // 1 when PP_CONV_NOEPI=1 is set: the halo and GEMM kernels skip the epilogue math and stores (main-loop-only timing)
 int pp_conv_noepi();
 

@@ -62,6 +62,8 @@ _SIGNATURES = {
     "pp_profile_enable": (_I, [_VP, _I]),
     "pp_profile_dump": (_I, [_VP, ctypes.c_char_p, _SZ]),
     "pp_op_conv": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _F, _VP, _VP, _VP]),
+    "pp_op_conv_ex": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _I, _VP, _I, _I, _VP, _I, _I, _VP,
+                           _I, _I, _VP]),
     "pp_op_corr_lookup": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
     "pp_op_conv_tf32": (_I, [_VP, _CP, _VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I,
                              _F, _F, _I, _VP, _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _VP]),
@@ -762,6 +764,25 @@ class Engine:
         out = torch.empty(N, OH, OW, m["cout_g"] * m["groups"], device=self.device, dtype=torch.float16)
         self._check(self.lib.pp_op_conv(self.h, name.encode(), _ptr(x_nhwc), N, H, W, stride, pad, dil, int(replicate),
                                         act, float(slope), _ptr(residual), _ptr(out), self._stream()))
+        return out
+
+    def op_conv_ex(self, name, x, out, x_co=0, out_co=0, pad=(0, 0), act=ACT_NONE, slope=0.0, scale=1.0, act2=ACT_NONE,
+                   residual=None, gru_zr=None, gru_h=None):
+        """One stride-1 fp16 convolution (weights from register_conv) of x [N,H,W,C] from channel x_co into out
+        [N,OH,OW,C'] from channel out_co.  Epilogue: act / slope / scale / act2 and an optional residual (tensor, co); or
+        gru_zr = (h, h_co, rh, rh_co) (z -> out, r * h -> rh); or gru_h = (h, h_co, z, z_co)."""
+        N, H, W, xC = x.shape
+        C = lambda t: 0 if t is None else t.shape[-1]
+        epi, a0, a0_co, a1, a1_co = self.EPI_STD, None, 0, None, 0
+        if residual is not None:
+            a0, a0_co = residual
+        if gru_zr is not None:
+            epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_ZR, gru_zr
+        if gru_h is not None:
+            epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_H, gru_h
+        self._check(self.lib.pp_op_conv_ex(
+            self.h, name.encode(), _ptr(x), xC, x_co, N, H, W, pad[0], pad[1], epi, act, float(slope), float(scale), act2,
+            _ptr(a0), C(a0), a0_co, _ptr(a1), C(a1), a1_co, _ptr(out), C(out), out_co, self._stream()))
         return out
 
     def op_corr_lookup(self, levels, coords, h8, w8):

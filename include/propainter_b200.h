@@ -170,6 +170,15 @@ PP_API int pp_profile_dump(pp_handle h, char* buf, size_t cap);
 /* Generic conv / linear through the wgmma implicit-GEMM kernel: x NHWC fp16 [N,H,W,cin_g*groups]. */
 PP_API int pp_op_conv(pp_handle h, const char* name, const void* x_f16, int N, int H, int W, int stride, int pad, int dil,
                int replicate, int act, float slope, const void* residual_f16, void* out_f16, void* stream);
+/* One stride-1 fp16 convolution into a channel slice: input x [N][H][W][x_C] from channel x_co (the layer's Cin, grouped
+ * layers read and write their groups packed), zero padding ph x pw, output out [N][OH][OW][out_C] from channel out_co,
+ * epilogue epi = 0: act2(act(acc + bias) * scale + aux0) with aux0 an optional residual [pix][aux0_C] at aux0_co;
+ * epi = 1 (GRU z|r): z -> out, r * aux0 (h) -> aux1 (r*h); epi = 2 (GRU q): (1 - z) * h + z * tanh(acc + bias) -> out
+ * with h = aux0, z = aux1. */
+PP_API int pp_op_conv_ex(pp_handle h, const char* name, const void* x_f16, int x_C, int x_co, int N, int H, int W, int ph,
+                         int pw, int epi, int act, float slope, float scale, int act2, const void* aux0_f16, int aux0_C,
+                         int aux0_co, void* aux1_f16, int aux1_C, int aux1_co, void* out_f16, int out_C, int out_co,
+                         void* stream);
 PP_API int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream);
 /* Operators of the fp32 RAFT and flow-completion paths (pp_raft_bidir_fp32, pp_flow_complete_fp32).  Split tensors are fp32 [pix][hi C | lo C] with hi = tf32(x),

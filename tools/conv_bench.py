@@ -2,7 +2,10 @@
 
 1x1 layers (linear layers and 1x1 convolutions) also report torch.nn.functional.linear (cuBLAS, fp16 with bias) on
 the same shape in the same process, as a yardstick for the flat GEMM kernel.  PP_CONV_NOEPI=1 in the environment skips
-the epilogue math and stores of the conv kernels (main-loop timing; the outputs are then garbage)."""
+the epilogue math and stores of the conv kernels (main-loop timing; the outputs are then garbage).
+
+EPI_CASES are the bench step's stride-1 layers with their real epilogues and output layouts (GRU gates, channel slices
+of the hidden-state tensor, residuals), run through Engine.op_conv_ex."""
 import math
 import sys
 import os
@@ -41,6 +44,54 @@ CASES = {
     "step conv (3x3, 128->128, M=7200)": (2, 45, 80, 128, 128, 3, 3, 1, 1),
     "step conv (3x3, 128->128, M=14400)": (1, 90, 160, 128, 128, 3, 3, 1, 1),
 }
+
+
+# name: (N, H, W, Cin, Cout, kh, kw, epilogue, output tensor width, output channel offset) at the shapes of one bench step
+# (80 frames at 640x360: RAFT at 1/8 resolution over 79 pairs per direction, the generator's encoder / propagation /
+# decoder).  Epilogues: "std" (bias + LReLU), "res" (+ residual), "zr" (GRU z | r * h), "h" (GRU (1 - z) h + z q, in place
+# in hx[:, 0:128]).
+EPI_CASES = {
+    "raft.gru.zr1 (1x5, 384->256, z | r*h)": (158, 45, 80, 384, 256, 1, 5, "zr", 128, 0),
+    "raft.gru.zr2 (5x1, 384->256, z | r*h)": (158, 45, 80, 384, 256, 5, 1, "zr", 128, 0),
+    "raft.gru.q1 (1x5, 384->128, in place)": (158, 45, 80, 384, 128, 1, 5, "h", 384, 0),
+    "raft.gru.q2 (5x1, 384->128, in place)": (158, 45, 80, 384, 128, 5, 1, "h", 384, 0),
+    "raft.convc2 (3x3, 256->192 into 256)": (158, 45, 80, 256, 192, 3, 3, "std", 256, 0),
+    "raft.convf2 (3x3, 128->64 into 256)": (158, 45, 80, 128, 64, 3, 3, "std", 256, 192),
+    "raft.update.conv (3x3, 256->126 into 384)": (158, 45, 80, 256, 126, 3, 3, "std", 384, 256),
+    "raft.fh1 (3x3, 128->256)": (158, 45, 80, 128, 256, 3, 3, "std", 256, 0),
+    "gen.fp.backbone.1 (3x3, 128->128 +res)": (20, 90, 160, 128, 128, 3, 3, "res", 128, 0),
+    "gen.encoder.8 (3x3, 256->384)": (80, 90, 160, 256, 384, 3, 3, "std", 384, 0),
+    "gen.decoder.4 (3x3, 64->64 @360x640)": (11, 360, 640, 64, 64, 3, 3, "std", 64, 0),
+}
+
+
+def _epi_case(eng, name, case, flush):
+    N, H, W, cin, cout, kh, kw, epi, out_c, out_co = case
+    w = torch.randn(cout, cin, kh, kw) / math.sqrt(cin * kh * kw)
+    eng.register_conv("b", w, torch.randn(cout) * 0.1, 1)
+    dev = "cuda:0"
+    x = torch.randn(N, H, W, cin, device=dev, dtype=torch.float16)
+    pad = (kh // 2, kw // 2)
+    kw_ = {}
+    if epi == "zr":
+        out = torch.empty(N, H, W, out_c, device=dev, dtype=torch.float16)
+        hx = torch.randn(N, H, W, 384, device=dev, dtype=torch.float16)
+        rh = torch.empty(N, H, W, 128, device=dev, dtype=torch.float16)
+        kw_["gru_zr"] = (hx, 0, rh, 0)
+    elif epi == "h":
+        out = torch.randn(N, H, W, out_c, device=dev, dtype=torch.float16)
+        z = torch.rand(N, H, W, 128, device=dev, dtype=torch.float16)
+        kw_["gru_h"] = (out, 0, z, 0)
+    else:
+        out = torch.empty(N, H, W, out_c, device=dev, dtype=torch.float16)
+        kw_.update(act=E.ACT_LRELU, slope=0.2)
+        if epi == "res":
+            kw_["residual"] = (torch.randn(N, H, W, cout, device=dev, dtype=torch.float16), 0)
+    fn = lambda: eng.op_conv_ex("b", x, out, out_co=out_co, pad=pad, **kw_)
+    ms = _time_ms(fn, flush)
+    fl = 2.0 * N * H * W * cout * cin * kh * kw
+    print(f"{name:42s} M={N * H * W:8d} bn={eng.conv_meta['b']['bn']:3d} {ms:8.3f} ms {fl / ms / 1e9:8.1f} TFLOP/s",
+          flush=True)
 
 
 def _time_ms(fn, flush, reps=5):
@@ -88,6 +139,10 @@ def main():
             del x2, w2, b2
         print(line, flush=True)
         del x, y
+    for name, case in EPI_CASES.items():
+        if only and not any(o in name for o in only):
+            continue
+        _epi_case(eng, name, case, flush)
 
 
 if __name__ == "__main__":
