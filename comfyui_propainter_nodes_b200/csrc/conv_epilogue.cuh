@@ -8,7 +8,7 @@ namespace ppconv {
 
 // ACC (the split-tf32 epilogue): fp32-accurate tanh (pp_common.cuh) instead of the fast-math tanh.approx, whose error is
 // below the fp16 storage rounding but far above fp32's
-// Works on any run of N values: 16 consecutive channels in conv_epilogue16, a fragment's 4 values in conv_gemm.cu.
+// Works on any run of N values: 16 consecutive channels in conv_epilogue16, a fragment's 4 values in frag_epilogue.
 template <int ACT, bool ACC = false, int N>
 __device__ __forceinline__ void act16_t(float (&v)[N], float slope) {
 #pragma unroll
@@ -66,9 +66,8 @@ __device__ __forceinline__ void store16(__half* dst, int nvalid, bool vec, const
 
 // `raw`: 16 fp32 accumulators (tile columns ng0-n0 .. +15) of output pixel `mrow` (flattened N*OH*OW index),
 // group g, first channel ng0 (within the group; ng0 < Cout_g).  `epi`/`vec` are launch-uniform.
-// The PP_EPI_STD branch's operation order is repeated per value by std_epi4 (the fragment epilogues of conv_gemm.cu and
-// conv_halo.cu), the GRU branches by conv_halo.cu's halo_frag_epilogue; keep them in step, a layer's results do not
-// depend on which kernel or epilogue path ran it.
+// frag_epilogue (below) repeats this operation order per value for every epilogue kind; keep the two in step, a layer's
+// results do not depend on which kernel or epilogue path ran it.
 __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uint32_t (&raw)[16], long long mrow, int g,
                                                 int ng0, int epi, bool vec) {
     const int nvalid = min(16, p.Cout_g - ng0);
@@ -141,25 +140,98 @@ __device__ __forceinline__ void conv_epilogue16(const PPConvParams& p, const uin
     }
 }
 
-// 4 accumulators of one fragment column pair (rows r and r + 8, columns c, c + 1) through the PP_EPI_STD epilogue, in
-// conv_epilogue16's operation order.  ACT1: p.act1 (dispatched once per tile, so the loop over the fragments has no
-// indirect branch); act2 is applied when set.  Used by the fragment epilogues of conv_gemm.cu and conv_halo.cu.
-template <int ACT1>
-__device__ __forceinline__ void std_epi4(float (&v)[4], bool has_bias, const float2& bias, float scale, bool has_res,
-                                          const float (&res)[4], int act2, float slope) {
-  if (has_bias) {
-    v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
+// ---- fragment epilogue of the TMA-store kernels (conv_gemm_kernel, conv_halo_kernel's TMA path)
+// A consumer warpgroup writes its rows of the tile as fp16 into a staging tile in shared memory, panels of PW channels
+// (64 / 32 / 16: 128B / 64B / 32B swizzle), each swizzled like the TMA box that stores it; panel P starts at P * PANEL.
+
+// Thread t128 copies the tile's bias columns 2 t128 and 2 t128 + 1 (bias channels goff + n0 + c, zero past Cout_g) to
+// `bs`: one coalesced load per thread instead of a dependent global load per fragment column.  goff: g * Cout_g.
+template <int BN>
+__device__ __forceinline__ void stage_bias(const PPConvParams& p, float* bs, int goff, int n0, int t128) {
+  const int c0 = 2 * t128, n = goff + n0 + c0;
+  float2 bv = make_float2(0.f, 0.f);
+  if (p.bias != nullptr && c0 < BN) {
+    if (n0 + c0 < p.Cout_g) bv.x = __ldg(p.bias + n);
+    if (n0 + c0 + 1 < p.Cout_g) bv.y = __ldg(p.bias + n + 1);
   }
-  act16_t<ACT1>(v, slope);
-  if (scale != 1.f) {
+  if (c0 < BN) *reinterpret_cast<float2*>(bs + c0) = bv;
+}
+
+// Byte offset of (row r, channel c % PW) within a panel: rows of PW * 2 bytes, the box swizzle XORs the 16-byte unit
+// index with the row's address bits 7.. (panels start 1024-byte aligned, so panel-relative bits are absolute ones).
+template <int PW>
+__device__ __forceinline__ int frag_stg_off(int r, int c) {
+  return r * PW * 2 + ((((c & (PW - 1)) >> 3) ^ ((r * PW * 2 >> 7) & (PW / 8 - 1))) << 4) + (c & 7) * 2;
+}
+
+// The fragment epilogue of one warpgroup into its staging tile `so`, in conv_epilogue16's operation order per value.
+// bs: the tile's bias columns (stage_bias).  STD: act1 is ACT1 (p.act1, dispatched once per tile, so the loop over the
+// fragments has no indirect branch), act2 is applied when set, and the residual (has_aux) is read from the staging tile
+// (TMA-loaded there) and overwritten in place.  GRU_ZR: sigmoid; r tiles multiply by h (in the staging tile).  GRU_H:
+// tanh, then (1 - z) h + z q with h in the staging tile and z in the warpgroup's z panel `zb`, which holds one panel at a
+// time: panel P of the tile reads it.  Every column of the tile (of panel P for GRU_H) is written, columns past Cout_g
+// are never stored, so the loop is straight-line code whose shared-memory accesses the compiler can batch.
+template <int MB, int BN, int PW, int PANEL, int EPI, int ACT1>
+__device__ __forceinline__ void frag_epilogue(const PPConvParams& p, const float (&acc)[MB][BN / 2], uint8_t* so,
+                                              const uint8_t* zb, const float* bs, bool has_aux, bool r_tile, int P,
+                                              int t128) {
+  const bool has_bias = p.bias != nullptr;
+  const float scale = p.scale, slope = p.slope;
+  const int act2 = p.act2;
+  // fragment of m64nNk16: register 4j + i of thread t holds row 16 * (t / 32) + (t % 32) / 4 + 8 * (i / 2), column
+  // 8j + 2 * (t % 4) + i % 2
+  const int fr = 16 * (t128 >> 5) + ((t128 & 31) >> 2), fc = 2 * (t128 & 3);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] *= scale;
-  }
-  if (has_res) {
+  for (int b = 0; b < MB; ++b) {
+    const int r = 64 * b + fr;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] += res[i];
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = 8 * j + fc;
+      if (EPI == PP_EPI_GRU_H && col / PW != P) continue;
+      // rows r and r + 8 differ above the swizzle's row bits
+      const int off = (col / PW) * PANEL + frag_stg_off<PW>(r, col);
+      __half2* lo = reinterpret_cast<__half2*>(so + off);
+      __half2* hi = reinterpret_cast<__half2*>(so + off + 8 * PW * 2);
+      const float2 bias = *reinterpret_cast<const float2*>(bs + col);
+      float v[4] = {acc[b][4 * j], acc[b][4 * j + 1], acc[b][4 * j + 2], acc[b][4 * j + 3]};
+      float a[4] = {0.f, 0.f, 0.f, 0.f};
+      if (has_aux) {
+        const float2 a0 = __half22float2(*lo), a1 = __half22float2(*hi);
+        a[0] = a0.x; a[1] = a0.y; a[2] = a1.x; a[3] = a1.y;
+      }
+      if (has_bias) {
+        v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
+      }
+      if constexpr (EPI == PP_EPI_STD) {
+        act16_t<ACT1>(v, slope);
+        if (scale != 1.f) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] *= scale;
+        }
+        if (has_aux) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] += a[i];
+        }
+        if (act2 != PP_ACT_NONE) act16(v, act2, slope);
+      } else if constexpr (EPI == PP_EPI_GRU_ZR) {
+        act16_t<PP_ACT_SIGMOID>(v, 0.f);
+        if (r_tile) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] *= a[i];
+        }
+      } else {
+        const int zoff = frag_stg_off<PW>(r, col);
+        const float2 z0 = __half22float2(*reinterpret_cast<const __half2*>(zb + zoff));
+        const float2 z1 = __half22float2(*reinterpret_cast<const __half2*>(zb + zoff + 8 * PW * 2));
+        const float z[4] = {z0.x, z0.y, z1.x, z1.y};
+        act16_t<PP_ACT_TANH>(v, 0.f);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[i] = (1.f - z[i]) * a[i] + z[i] * v[i];
+      }
+      *lo = __floats2half2_rn(v[0], v[1]);
+      *hi = __floats2half2_rn(v[2], v[3]);
+    }
   }
-  if (act2 != PP_ACT_NONE) act16(v, act2, slope);
 }
 
 // ---- split-tf32 form (PPConvParams::split): fp32 [hi | lo] operands, see conv_igemm.cuh

@@ -8,9 +8,10 @@
 //     with Cout <= 128, 256 x 128 (MB = 2: two m64 blocks of 128 columns), 128 accumulator registers per thread either
 //     way.  Per 64-channel K chunk a stage holds the A rows (one 2-D TMA box per segment view, zero-filled past M and
 //     past the last segment's channels) and the pre-swizzled weight tile (cp.async.bulk), 48 KB in both shapes.
-//   * the epilogue runs on the wgmma fragments: bias, act1, scale, residual, act2 in the order of conv_epilogue16's
-//     PP_EPI_STD branch, fp16 into a 128B-swizzled staging tile from which one thread per warpgroup issues TMA stores
-//     (rows / columns past the tensor are clipped).  The stores drain while the next tile's main loop runs; the staging
+//   * the epilogue runs on the wgmma fragments (ppconv::frag_epilogue, shared with conv_halo_kernel's TMA path): bias,
+//     act1, scale, residual, act2 in the order of conv_epilogue16's PP_EPI_STD branch, fp16 into a 128B-swizzled
+//     staging tile of 64-channel panels that span both warpgroups' rows, from which one thread per warpgroup issues TMA
+//     stores (rows / columns past the tensor are clipped).  The stores drain while the next tile's main loop runs; the staging
 //     tile is only waited for (cp.async.bulk.wait_group.read) before it is written again.  A residual tile (the in-place
 //     transformer proj) is TMA-loaded into the staging tile, read and overwritten in place by the same threads.
 //     The tile's bias columns are copied to shared memory once per tile and act1 is a compile-time case, so the loop
@@ -63,43 +64,6 @@ __device__ __forceinline__ Smem gemm_smem() {
   return m;
 }
 
-// The fragment epilogue of one warpgroup into its rows of the staging tile `so`.  Every column of the tile is written
-// (the staging tile has room for all of them; columns past Cout_g are never stored), so the loop is straight-line code
-// whose shared-memory loads and stores the compiler can batch.
-template <int MB, int BN, int ACT1>
-__device__ __forceinline__ void gemm_epilogue(const PPConvParams& p, const float (&acc)[MB][BN / 2], uint8_t* so,
-                                              const float* bs, bool has_res, int t128) {
-  constexpr int PANEL = 128 * MB * 128;
-  const bool has_bias = p.bias != nullptr;
-  const float scale = p.scale, slope = p.slope;
-  const int act2 = p.act2;
-  // fragment of m64nNk16: register 4j + i of thread t holds row 16 * (t / 32) + (t % 32) / 4 + 8 * (i / 2), column
-  // 8j + 2 * (t % 4) + i % 2
-  const int fr = 16 * (t128 >> 5) + ((t128 & 31) >> 2), fc = 2 * (t128 & 3);
-#pragma unroll
-  for (int b = 0; b < MB; ++b) {
-    const int r = 64 * b + fr;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = 8 * j + fc;
-      // 128B swizzle: the 16-byte unit (col % 64) / 8 of row r sits at unit index XOR (r & 7); (r + 8) & 7 == r & 7
-      const int off = (col >> 6) * PANEL + r * 128 + (((((col & 63) >> 3) ^ (r & 7))) << 4) + (col & 7) * 2;
-      __half2* lo = reinterpret_cast<__half2*>(so + off);
-      __half2* hi = reinterpret_cast<__half2*>(so + off + 8 * 128);
-      const float2 bias = *reinterpret_cast<const float2*>(bs + col);
-      float v[4] = {acc[b][4 * j], acc[b][4 * j + 1], acc[b][4 * j + 2], acc[b][4 * j + 3]};
-      float res[4] = {0.f, 0.f, 0.f, 0.f};
-      if (has_res) {
-        const float2 r0 = __half22float2(*lo), r1 = __half22float2(*hi);
-        res[0] = r0.x; res[1] = r0.y; res[2] = r1.x; res[3] = r1.y;
-      }
-      ppconv::std_epi4<ACT1>(v, has_bias, bias, scale, has_res, res, act2, slope);
-      *lo = __floats2half2_rn(v[0], v[1]);
-      *hi = __floats2half2_rn(v[2], v[3]);
-    }
-  }
-}
-
 // One tile of one consumer warpgroup: main loop into acc[MB][BN / 2], then the fragment epilogue into the staging tile
 // and this warpgroup's TMA stores.  The ring position (s, ph) runs on across tiles.
 template <int MB, int BN>
@@ -143,18 +107,9 @@ __device__ __forceinline__ void gemm_tile(const GemmParams& h, const Smem& m, in
   const int npanel = (min(BN, p.Cout_g - n0) + 63) / 64;
   uint8_t* so = m.out + wg * WG_ROWS * 128;
   const bool issuer = t128 == 0;
-  // the tile's bias columns (one coalesced load per thread instead of a dependent load per fragment column); the
-  // previous tile's readers of this copy have passed its last named barrier
+  // the tile's bias columns; the previous tile's readers of this copy have passed its last named barrier
   float* bs = m.bias + wg * 256;
-  {
-    const int c0 = 2 * t128, n = n0 + c0;
-    float2 bv = make_float2(0.f, 0.f);
-    if (p.bias != nullptr && c0 < BN) {
-      if (n < p.Cout_g) bv.x = __ldg(p.bias + n);
-      if (n + 1 < p.Cout_g) bv.y = __ldg(p.bias + n + 1);
-    }
-    if (c0 < BN) *reinterpret_cast<float2*>(bs + c0) = bv;
-  }
+  ppconv::stage_bias<BN>(p, bs, 0, n0, t128);
   if (issuer) tma_store_wait_read<0>();   // the previous tile's stores have read it
   named_bar(bar_id, 128);
   const bool has_res = p.aux0 != nullptr;
@@ -166,13 +121,18 @@ __device__ __forceinline__ void gemm_tile(const GemmParams& h, const Smem& m, in
     mbar_wait(&m.res[wg], rph);
     rph ^= 1;
   }
+  // 64-channel panels of all the tile's rows (both warpgroups')
+  auto epilogue = [&](auto act1) {
+    ppconv::frag_epilogue<MB, BN, 64, PANEL, PP_EPI_STD, decltype(act1)::value>(p, acc, so, nullptr, bs, has_res, false, 0,
+                                                                                t128);
+  };
   switch (p.act1) {
-    case PP_ACT_RELU: gemm_epilogue<MB, BN, PP_ACT_RELU>(p, acc, so, bs, has_res, t128); break;
-    case PP_ACT_LRELU: gemm_epilogue<MB, BN, PP_ACT_LRELU>(p, acc, so, bs, has_res, t128); break;
-    case PP_ACT_SIGMOID: gemm_epilogue<MB, BN, PP_ACT_SIGMOID>(p, acc, so, bs, has_res, t128); break;
-    case PP_ACT_TANH: gemm_epilogue<MB, BN, PP_ACT_TANH>(p, acc, so, bs, has_res, t128); break;
-    case PP_ACT_GELU: gemm_epilogue<MB, BN, PP_ACT_GELU>(p, acc, so, bs, has_res, t128); break;
-    default: gemm_epilogue<MB, BN, PP_ACT_NONE>(p, acc, so, bs, has_res, t128); break;
+    case PP_ACT_RELU: epilogue(ppconv::IntC<PP_ACT_RELU>{}); break;
+    case PP_ACT_LRELU: epilogue(ppconv::IntC<PP_ACT_LRELU>{}); break;
+    case PP_ACT_SIGMOID: epilogue(ppconv::IntC<PP_ACT_SIGMOID>{}); break;
+    case PP_ACT_TANH: epilogue(ppconv::IntC<PP_ACT_TANH>{}); break;
+    case PP_ACT_GELU: epilogue(ppconv::IntC<PP_ACT_GELU>{}); break;
+    default: epilogue(ppconv::IntC<PP_ACT_NONE>{}); break;
   }
   fence_proxy_async();           // generic-proxy smem writes -> visible to the TMA store
   named_bar(bar_id, 128);
@@ -239,10 +199,6 @@ int gemm_mb(const PPConvParams& p) { return p.Cout_g_pad <= 128 && p.M_total >= 
 
 long long gemm_tiles(const PPConvParams& p, int mb) {
   return pp_ceil_div64(p.M_total, 128 * mb) * pp_ceil_div(p.Cout_g_pad, 256 / mb);
-}
-
-bool aligned16(const void* ptr, int cstride, int coff) {
-  return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cstride % 8 == 0 && coff % 8 == 0;
 }
 
 }  // namespace

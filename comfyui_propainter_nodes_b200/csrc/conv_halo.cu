@@ -18,12 +18,14 @@
 // then the fused epilogue of conv_epilogue.cuh -> global), warp 8 patch producer (TMA), warp 9 weight producer (bulk
 // copy).  MT == 1: warpgroup w owns pixel rows 64w..64w+63 of the sub-tile; MT == 2: warpgroup w owns sub-tile w.
 //
-// Epilogue.  conv_halo_kernel runs it on the wgmma fragments where the layer's output can be TMA-stored (fp16, 16-byte
-// aligned; halo_tma_configure): the tile's bias columns are copied to shared memory once, act1 is a compile-time case,
-// the residual / GRU h / GRU z operands are TMA-loaded into shared memory while the tile's last wgmmas run, results go
-// as fp16 into a swizzled staging tile that one thread per warpgroup TMA-stores, and the stores drain under the next
-// tile's main loop.  Every other layer, and the other two kernels, copy the accumulators through an fp32 staging tile 32
-// columns at a time into conv_epilogue16 (drain_acc), which loads its operands and stores per thread.
+// Epilogue.  All three kernels share one main loop (halo_mainloop).  conv_halo_kernel runs the epilogue on the wgmma
+// fragments where the layer's output can be TMA-stored (fp16, 16-byte aligned; halo_tma_configure): the tile's bias
+// columns are copied to shared memory once, act1 is a compile-time case, the residual / GRU h / GRU z operands are
+// TMA-loaded into shared memory while the tile's last wgmmas run, results go as fp16 into a swizzled staging tile
+// (ppconv::frag_epilogue, shared with conv_gemm.cu) that one thread per warpgroup TMA-stores, and the stores drain under
+// the next tile's main loop.  Every other layer, and the other two kernels, copy the accumulators through an fp32 staging
+// tile 32 columns at a time into conv_epilogue16 (drain_acc), which loads its operands and stores per thread.  The
+// shared-memory plan (halo_smem) is the same for both, with an epilogue region of the epilogue's size.
 //
 // conv_halo_tf32_kernel is the split-tf32 form (PPConvParams::split, see conv_igemm.cuh): the byte geometry is the same
 // (a 128-byte swizzled K-chunk row holds 32 fp32 channels, each chunk is 4 wgmmas m64nNk8 with the same 32-byte
@@ -44,10 +46,12 @@ constexpr int NUM_THREADS = 384;   // warpgroup 2: warps 8-9 producers, 10-11 id
 constexpr int NUM_EPI_THREADS = 256;   // the two consumer warpgroups
 constexpr int WARP_A = 8, WARP_B = 9;
 constexpr int MAX_SA = 4, MAX_SB = 8;
-// stages; the accumulator staging tiles of the epilogue (2 x ppconv::STG_BYTES) and the barrier block come on top (see
-// HaloSmem)
+// stages of the layers on the drain epilogue; the rest of the plan comes on top (halo_smem)
 constexpr int SMEM_BUDGET = 186 * 1024;
 constexpr int SMEM_MAX = 227 * 1024;   // dynamic shared memory of one CTA on sm_90
+constexpr int SMEM_ALIGN_SLACK = 1024;   // dyn_smem_1024 moves the base up to a 1024-byte boundary
+constexpr int BAR_BLOCK_BYTES = 1024;    // the barriers; keeps the epilogue region behind it 1024-byte aligned
+constexpr int DRAIN_EPI_BYTES = 2 * ppconv::STG_BYTES;   // the drain epilogue's fp32 staging tile per consumer warpgroup
 
 struct HaloLayer {
   PPConvParams c;
@@ -101,21 +105,22 @@ struct Ring {
 };
 
 // Shared-memory carve-up of the halo kernels, from the 1024-byte aligned base:
-//   SA patch stages | SB weight stages | barrier block (1 KB) | 2 accumulator staging tiles
-// (conv_halo_kernel's TMA epilogue puts its own region in place of the staging tiles, see halo_tma_region_bytes)
-// The launchers call it with base == nullptr and read only `bytes`.
+//   SA patch stages | SB weight stages | barrier block | epilogue region of epi_bytes
+// The region holds the drain's fp32 staging tiles (DRAIN_EPI_BYTES) or conv_halo_kernel's TMA epilogue
+// (halo_tma_region_bytes).  The launchers call it with base == nullptr and read only `bytes`.
 struct HaloSmem {
   uint8_t* a;                  // patch stages (TMA, 128B swizzle: 1024-byte aligned)
   uint8_t* b;                  // weight stages
   int SA, SB, a_stage_bytes, b_stage_bytes;
   uint64_t *a_full, *a_empty, *b_full, *b_empty;
   uint64_t* spare;             // one more barrier (conv_prog_kernel: layer_go)
-  float* acc_stg;              // ppconv::STG_BYTES per consumer warpgroup
+  uint8_t* epi;                // the epilogue region
   int bytes;                   // dynamic shared memory, including the slack that aligns the base
 };
 
-__host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage_bytes, int SB, int b_stage_bytes) {
-  const int b_off = SA * a_stage_bytes, bar_off = b_off + SB * b_stage_bytes, acc_off = bar_off + 1024;
+__host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage_bytes, int SB, int b_stage_bytes,
+                                              int epi_bytes) {
+  const int b_off = SA * a_stage_bytes, bar_off = b_off + SB * b_stage_bytes, epi_off = bar_off + BAR_BLOCK_BYTES;
   HaloSmem m;
   m.SA = SA; m.SB = SB; m.a_stage_bytes = a_stage_bytes; m.b_stage_bytes = b_stage_bytes;
   m.a = base;
@@ -125,8 +130,8 @@ __host__ __device__ inline HaloSmem halo_smem(uint8_t* base, int SA, int a_stage
   m.b_full = m.a_empty + MAX_SA;
   m.b_empty = m.b_full + MAX_SB;
   m.spare = m.b_empty + MAX_SB;
-  m.acc_stg = reinterpret_cast<float*>(base + acc_off);
-  m.bytes = 1024 + acc_off + 2 * ppconv::STG_BYTES;
+  m.epi = base + epi_off;
+  m.bytes = SMEM_ALIGN_SLACK + epi_off + epi_bytes;
   return m;
 }
 
@@ -174,16 +179,12 @@ __device__ __forceinline__ void halo_tap_group(int tn, float (&acc)[MB][BN / 2],
   wgmma_commit();
 }
 
-// Consumer side of one tile, run by each of the two consumer warpgroups: the main loop into register accumulators
-// (MB = h.MT m64 blocks of BN columns), then the epilogue of this warpgroup's pixel rows.  A stage is handed back to
-// its producer once the wgmma group that read it has completed (one group per weight stage, one group in flight).
-// NT: see halo_tap_group.  TF32: the split-tf32 form.  PROG (conv_prog_kernel): the layer has the plain epilogue
-// (PP_EPI_STD), so the GRU epilogues are not compiled in.
-// The main loop of halo_tile into acc, for conv_halo_kernel's TMA epilogue: `before_wait` runs once the tile's last
-// commit group is issued, before the wait for it (the epilogue issues its operand loads there).  halo_tile keeps its
-// own copy of the loop so that the kernels on the drain epilogue (conv_prog_kernel, conv_halo_tf32_kernel) compile
-// to the same code as before.
-template <int BN, int MB, int NT, class BeforeWait>
+// The main loop of one tile, run by each of the two consumer warpgroups: into register accumulators acc (MB = h.MT m64
+// blocks of BN columns).  A stage is handed back to its producer once the wgmma group that read it has completed (one
+// group per weight stage, one group in flight).  NT: see halo_tap_group.  TF32: the split-tf32 form.  `before_wait`
+// runs once the tile's last commit group is issued, before the wait for it (the TMA epilogue issues its operand loads
+// there).
+template <int BN, int MB, int NT, bool TF32, class BeforeWait>
 __device__ __forceinline__ void halo_mainloop(const HaloLayer& h, const HaloSmem& m, Ring& ra, Ring& rb, int wg,
                                               float (&acc)[MB][BN / 2], BeforeWait&& before_wait) {
   using namespace ppx;
@@ -208,7 +209,7 @@ __device__ __forceinline__ void halo_mainloop(const HaloLayer& h, const HaloSmem
     for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
       mbar_wait(&m.b_full[rb.s], rb.ph);
       const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(m.b + rb.s * m.b_stage_bytes));
-      halo_tap_group<BN, MB, NT, false>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
+      halo_tap_group<BN, MB, NT, TF32>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
       wgmma_wait<1>();
       if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
       if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
@@ -226,50 +227,18 @@ __device__ __forceinline__ void halo_mainloop(const HaloLayer& h, const HaloSmem
   if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
 }
 
+// One tile of one consumer warpgroup on the drain epilogue: the main loop, then the epilogue of this warpgroup's pixel
+// rows through the fp32 staging tile `stg`.  TF32: the split-tf32 form.  PROG (conv_prog_kernel): the layer has the
+// plain epilogue (PP_EPI_STD), so the GRU epilogues are not compiled in.
 template <int BN, int MB, int NT, bool TF32 = false, bool PROG = false>
 __device__ __forceinline__ void halo_tile(const HaloLayer& h, int tile, const HaloSmem& m, Ring& ra, Ring& rb, float* stg,
                                           int wg, int t128) {
-  using namespace ppx;
   const PPConvParams& p = h.c;
-  const int taps = p.kh * p.kw;
   const TileCoord t = decode_tile(h, tile);
   const int n0 = t.n_idx * p.BN;
   const int bnt = min(p.BN, p.Cout_g_pad - n0);   // columns >= bnt of the last N tile read stale weights: never stored
-  const uint32_t sbo = h.flat ? 1024u : (uint32_t)h.BW * 128;
-  const uint32_t step_x = (uint32_t)p.dw * 8;                                 // next tap in the row (16-byte units)
-  const uint32_t step_row = (uint32_t)(p.dh * h.BW - (p.kw - 1) * p.dw) * 8;  // last tap of a row -> next row
-  const uint32_t tap16 = (uint32_t)p.BN * 8;                                  // next tap's weight tile in the stage
-  const int kw = p.kw;
-  uint32_t aoff[MB];
-#pragma unroll
-  for (int b = 0; b < MB; ++b) aoff[b] = MB == 2 ? wg * h.sub_bytes + b * 8 * sbo : wg * 8 * sbo;
   float acc[MB][BN / 2];
-  uint32_t accum = 0;
-  int pend_a = -1, pend_b = -1;
-  for (int c = 0; c < h.chunks; ++c) {
-    mbar_wait(&m.a_full[ra.s], ra.ph);
-    uint64_t adesc[MB];
-#pragma unroll
-    for (int b = 0; b < MB; ++b) adesc[b] = gmma_desc_sw128_kmajor(smem_u32(m.a + ra.s * m.a_stage_bytes) + aoff[b], sbo);
-    int kx = 0;
-    for (int tap0 = 0; tap0 < taps; tap0 += h.tps) {
-      mbar_wait(&m.b_full[rb.s], rb.ph);
-      const uint64_t bdesc = gmma_desc_sw128_kmajor(smem_u32(m.b + rb.s * m.b_stage_bytes));
-      halo_tap_group<BN, MB, NT, TF32>(min(h.tps, taps - tap0), acc, adesc, bdesc, accum, kx, kw, step_x, step_row, tap16);
-      wgmma_wait<1>();
-      if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
-      if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
-      pend_b = rb.s;
-      pend_a = tap0 + h.tps >= taps ? ra.s : -1;
-      if (++rb.s == m.SB) { rb.s = 0; rb.ph ^= 1; }
-    }
-    if (++ra.s == m.SA) { ra.s = 0; ra.ph ^= 1; }
-  }
-  wgmma_wait<0>();
-#pragma unroll
-  for (int b = 0; b < MB; ++b) wgmma_fence_acc(acc[b]);
-  if (pend_b >= 0) mbar_arrive(&m.b_empty[pend_b]);
-  if (pend_a >= 0) mbar_arrive(&m.a_empty[pend_a]);
+  halo_mainloop<BN, MB, NT, TF32>(h, m, ra, rb, wg, acc, [] {});
 
   // ---- epilogue
   const bool skip = (h.debug & 1) != 0;
@@ -295,10 +264,10 @@ __device__ __forceinline__ void halo_tile(const HaloLayer& h, int tile, const Ha
 }
 
 // ---- conv_halo_kernel's TMA epilogue (HaloParams::tma_out)
-// After the barrier block, in place of the drain's fp32 staging tiles:
+// Its epilogue region (HaloSmem::epi):
 //   fp16 staging tile | the tile's bias columns | GRU_H: one z panel per warpgroup
-// The staging tile holds, per consumer warpgroup, BN / pw panels of [64 MT pixels][pw channels], each swizzled like the
-// TMA box that stores it (128B / 64B / 32B swizzle for 64 / 32 / 16 channels).  A warpgroup's pixels are its 8 x 16
+// The staging tile holds, per consumer warpgroup, BN / pw panels of [64 MT pixels][pw channels] (ppconv::frag_epilogue
+// with PW = pw and a panel stride of one warpgroup's rows).  A warpgroup's pixels are its 8 x 16
 // (MT = 2) or 8 x 8 (MT = 1) block of the tile, or its run of consecutive pixels in flat mode, in box order, so row r of
 // a panel is accumulator row r of the warpgroup.
 __host__ __device__ constexpr int halo_panel_width(int bn) { return bn % 64 == 0 ? 64 : bn % 32 == 0 ? 32 : 16; }
@@ -308,78 +277,12 @@ __host__ __device__ constexpr int halo_out_z_bytes(int mt, int bn) { return 2 * 
 __host__ __device__ constexpr int halo_tma_region_bytes(int mt, int bn, bool gru_h) {
   return halo_out_stage_bytes(mt, bn) + halo_out_bias_bytes(bn) + (gru_h ? halo_out_z_bytes(mt, bn) : 0);
 }
+// the epilogue region of a conv_halo_kernel / conv_halo_tf32_kernel launch
+__host__ __device__ inline int halo_epi_bytes(const HaloParams& h) {
+  return h.tma_out ? halo_tma_region_bytes(h.MT, h.c.BN, h.c.epi == PP_EPI_GRU_H) : DRAIN_EPI_BYTES;
+}
 // barriers of the operand loads, one per consumer warpgroup, behind HaloSmem::spare
 __device__ __forceinline__ uint64_t* halo_out_bar(const HaloSmem& m, int wg) { return m.spare + 1 + wg; }
-
-// Byte offset of (row r, channel c % PW) within a panel: rows of PW * 2 bytes, the box swizzle XORs the 16-byte unit
-// index with address bits 7.. (panels start 1024-byte aligned, so panel-relative bits are absolute ones)
-template <int PW>
-__device__ __forceinline__ uint32_t halo_stg_off(int r, int c) {
-  const uint32_t off = (uint32_t)(r * PW * 2 + (c % PW) * 2);
-  return off ^ ((off >> 3) & (uint32_t)((PW / 8 - 1) << 4));
-}
-
-// The fragment epilogue of one warpgroup into its staging tile `so` (conv_epilogue16's operation order per value).
-// STD: std_epi4, the residual read from the staging tile (TMA-loaded there) and overwritten in place.  GRU_ZR: sigmoid;
-// r tiles multiply by h (in the staging tile).  GRU_H: tanh, then (1 - z) h + z q with h in the staging tile and z in the
-// warpgroup's z panel `zb`, which holds one panel at a time: panel P of the tile reads it.
-template <int MB, int BN, int EPI, int ACT1>
-__device__ __forceinline__ void halo_frag_epilogue(const PPConvParams& p, const float (&acc)[MB][BN / 2], uint8_t* so,
-                                                   const uint8_t* zb, const float* bs, bool has_aux, bool r_tile, int P,
-                                                   int t128) {
-  constexpr int PW = halo_panel_width(BN);
-  constexpr int PANEL = 64 * MB * PW * 2;
-  const bool has_bias = p.bias != nullptr;
-  const float scale = p.scale, slope = p.slope;
-  const int act2 = p.act2;
-  // fragment of m64nNk16: register 4j + i of thread t holds row 16 * (t / 32) + (t % 32) / 4 + 8 * (i / 2), column
-  // 8j + 2 * (t % 4) + i % 2
-  const int fr = 16 * (t128 >> 5) + ((t128 & 31) >> 2), fc = 2 * (t128 & 3);
-#pragma unroll
-  for (int b = 0; b < MB; ++b) {
-    const int r = 64 * b + fr;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = 8 * j + fc;
-      if (EPI == PP_EPI_GRU_H && col / PW != P) continue;
-      // rows r and r + 8 differ above the swizzle's row bits
-      const uint32_t off = (col / PW) * PANEL + halo_stg_off<PW>(r, col);
-      __half2* lo = reinterpret_cast<__half2*>(so + off);
-      __half2* hi = reinterpret_cast<__half2*>(so + off + 8 * PW * 2);
-      const float2 bias = *reinterpret_cast<const float2*>(bs + col);
-      float v[4] = {acc[b][4 * j], acc[b][4 * j + 1], acc[b][4 * j + 2], acc[b][4 * j + 3]};
-      float a[4] = {0.f, 0.f, 0.f, 0.f};
-      if (has_aux) {
-        const float2 a0 = __half22float2(*lo), a1 = __half22float2(*hi);
-        a[0] = a0.x; a[1] = a0.y; a[2] = a1.x; a[3] = a1.y;
-      }
-      if constexpr (EPI == PP_EPI_STD) {
-        ppconv::std_epi4<ACT1>(v, has_bias, bias, scale, has_aux, a, act2, slope);
-      } else {
-        if (has_bias) {
-          v[0] += bias.x; v[1] += bias.y; v[2] += bias.x; v[3] += bias.y;
-        }
-        if constexpr (EPI == PP_EPI_GRU_ZR) {
-          ppconv::act16_t<PP_ACT_SIGMOID>(v, 0.f);
-          if (r_tile) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) v[i] *= a[i];
-          }
-        } else {
-          const uint32_t zoff = halo_stg_off<PW>(r, col);
-          const float2 z0 = __half22float2(*reinterpret_cast<const __half2*>(zb + zoff));
-          const float2 z1 = __half22float2(*reinterpret_cast<const __half2*>(zb + zoff + 8 * PW * 2));
-          const float z[4] = {z0.x, z0.y, z1.x, z1.y};
-          ppconv::act16_t<PP_ACT_TANH>(v, 0.f);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) v[i] = (1.f - z[i]) * a[i] + z[i] * v[i];
-        }
-      }
-      *lo = __floats2half2_rn(v[0], v[1]);
-      *hi = __floats2half2_rn(v[2], v[3]);
-    }
-  }
-}
 
 // One tile of one consumer warpgroup on the TMA path: the main loop; the operand loads of the epilogue (residual / h
 // into the staging tile, GRU_H's first z panel) issued once the last commit group is out, so they overlap its wgmmas;
@@ -400,9 +303,9 @@ __device__ __forceinline__ void halo_tile_tma(const HaloParams& h, int tile, con
   const bool r_tile = epi == PP_EPI_GRU_ZR && n0 >= half_c;   // GRU_ZR: BN divides half_c (halo_tma_configure)
   const bool has_aux = epi == PP_EPI_STD ? p.aux0 != nullptr : (epi == PP_EPI_GRU_H || r_tile);
   const int npanel = (min(BN, p.Cout_g - n0) + PW - 1) / PW;   // panels with channels to store; TMA clips the last one
-  uint8_t* so = reinterpret_cast<uint8_t*>(m.acc_stg) + wg * (64 * MB * BN * 2);
-  float* bs = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(m.acc_stg) + halo_out_stage_bytes(MB, BN)) + wg * BN;
-  uint8_t* zb = reinterpret_cast<uint8_t*>(bs - wg * BN) + halo_out_bias_bytes(BN) + wg * PANEL;
+  uint8_t* so = m.epi + wg * (64 * MB * BN * 2);
+  float* bs = reinterpret_cast<float*>(m.epi + halo_out_stage_bytes(MB, BN)) + wg * BN;
+  uint8_t* zb = m.epi + halo_out_stage_bytes(MB, BN) + halo_out_bias_bytes(BN) + wg * PANEL;
   uint64_t* xbar = halo_out_bar(m, wg);
   // this warpgroup's box: pixel coordinates (flat: first pixel) and image
   int x0, y0, img;
@@ -415,7 +318,7 @@ __device__ __forceinline__ void halo_tile_tma(const HaloParams& h, int tile, con
   const bool issuer = t128 == 0;
   const bool skip = (h.debug & 1) != 0;
   float acc[MB][BN / 2];
-  halo_mainloop<BN, MB, NT>(h, m, ra, rb, wg, acc, [&] {
+  halo_mainloop<BN, MB, NT, false>(h, m, ra, rb, wg, acc, [&] {
     if (issuer && has_aux && !skip) {
       tma_store_wait_read<0>();   // the previous tile's stores have read the staging tile
       const int nz = epi == PP_EPI_GRU_H ? 1 : 0;
@@ -428,15 +331,7 @@ __device__ __forceinline__ void halo_tile_tma(const HaloParams& h, int tile, con
   if (skip) return;
 
   // the tile's bias columns; the previous tile's readers of this copy have passed its last named barrier
-  {
-    const int c0 = 2 * t128, n = t.g * p.Cout_g + n0 + c0;
-    float2 bv = make_float2(0.f, 0.f);
-    if (p.bias != nullptr && c0 < BN) {
-      if (n0 + c0 < p.Cout_g) bv.x = __ldg(p.bias + n);
-      if (n0 + c0 + 1 < p.Cout_g) bv.y = __ldg(p.bias + n + 1);
-    }
-    if (c0 < BN) *reinterpret_cast<float2*>(bs + c0) = bv;
-  }
+  ppconv::stage_bias<BN>(p, bs, t.g * p.Cout_g, n0, t128);
   const int bar_id = 4 + wg;
   if (issuer && !has_aux) tma_store_wait_read<0>();
   named_bar(bar_id, 128);
@@ -444,14 +339,19 @@ __device__ __forceinline__ void halo_tile_tma(const HaloParams& h, int tile, con
     mbar_wait(xbar, xph);
     xph ^= 1;
   }
+  using ppconv::IntC;
+  auto epilogue = [&](auto kind, auto act1, bool aux, int P) {
+    ppconv::frag_epilogue<MB, BN, PW, PANEL, decltype(kind)::value, decltype(act1)::value>(p, acc, so, zb, bs, aux, r_tile,
+                                                                                           P, t128);
+  };
   if (epi == PP_EPI_STD) {
     switch (p.act1) {
-      case PP_ACT_RELU: halo_frag_epilogue<MB, BN, PP_EPI_STD, PP_ACT_RELU>(p, acc, so, zb, bs, has_aux, false, 0, t128); break;
-      case PP_ACT_LRELU: halo_frag_epilogue<MB, BN, PP_EPI_STD, PP_ACT_LRELU>(p, acc, so, zb, bs, has_aux, false, 0, t128); break;
-      default: halo_frag_epilogue<MB, BN, PP_EPI_STD, PP_ACT_NONE>(p, acc, so, zb, bs, has_aux, false, 0, t128); break;
+      case PP_ACT_RELU: epilogue(IntC<PP_EPI_STD>{}, IntC<PP_ACT_RELU>{}, has_aux, 0); break;
+      case PP_ACT_LRELU: epilogue(IntC<PP_EPI_STD>{}, IntC<PP_ACT_LRELU>{}, has_aux, 0); break;
+      default: epilogue(IntC<PP_EPI_STD>{}, IntC<PP_ACT_NONE>{}, has_aux, 0); break;
     }
   } else if (epi == PP_EPI_GRU_ZR) {
-    halo_frag_epilogue<MB, BN, PP_EPI_GRU_ZR, PP_ACT_NONE>(p, acc, so, zb, bs, r_tile, r_tile, 0, t128);
+    epilogue(IntC<PP_EPI_GRU_ZR>{}, IntC<PP_ACT_NONE>{}, r_tile, 0);
   } else {
     // one z panel at a time: before the next one is loaded, every thread has read the current one
 #pragma unroll 1
@@ -465,7 +365,7 @@ __device__ __forceinline__ void halo_tile_tma(const HaloParams& h, int tile, con
         mbar_wait(xbar, xph);
         xph ^= 1;
       }
-      halo_frag_epilogue<MB, BN, PP_EPI_GRU_H, PP_ACT_NONE>(p, acc, so, zb, bs, true, false, pn, t128);
+      epilogue(IntC<PP_EPI_GRU_H>{}, IntC<PP_ACT_NONE>{}, true, pn);
     }
   }
   fence_proxy_async();           // generic-proxy smem writes -> visible to the TMA stores
@@ -546,7 +446,7 @@ __device__ __forceinline__ void halo_produce_weights(const HaloLayer& h, const H
 template <bool TF32>
 __device__ __forceinline__ void halo_body(const HaloParams& h) {
   using namespace ppx;
-  const HaloSmem m = halo_smem(dyn_smem_1024(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes);
+  const HaloSmem m = halo_smem(dyn_smem_1024(), h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, halo_epi_bytes(h));
   const int tid = threadIdx.x, warp = tid >> 5;
   if (tid == 0) {
     if constexpr (!TF32) {
@@ -566,7 +466,7 @@ __device__ __forceinline__ void halo_body(const HaloParams& h) {
   if (warp < 8) {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue
     const int wg = tid >> 7, t128 = tid & 127;
-    float* stg = m.acc_stg + wg * (ppconv::STG_BYTES / 4);
+    float* stg = reinterpret_cast<float*>(m.epi + wg * ppconv::STG_BYTES);
     Ring ra = {0, 0}, rb = {0, 0};
     const int total_tiles = halo_total_tiles(h);
     if constexpr (!TF32) {
@@ -671,7 +571,7 @@ __device__ __forceinline__ void prog_wait(const unsigned int* counter, unsigned 
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_constant__ ProgParams P) {
   using namespace ppx;
-  const HaloSmem m = halo_smem(dyn_smem_1024(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes);
+  const HaloSmem m = halo_smem(dyn_smem_1024(), P.SA, P.a_stage_bytes, P.SB, P.b_stage_bytes, DRAIN_EPI_BYTES);
   uint64_t* layer_go = m.spare;   // the CTA's one poller (TMA producer thread) -> consumers: layer li may start
 
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -689,7 +589,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_prog_kernel(const __grid_
   if (warp < 8) {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue (+ the sampling layers)
     const int wg = tid >> 7, t128 = tid & 127;
-    float* stg = m.acc_stg + wg * (ppconv::STG_BYTES / 4);
+    float* stg = reinterpret_cast<float*>(m.epi + wg * ppconv::STG_BYTES);
     Ring ra = {0, 0}, rb = {0, 0};
     for (int li = 0; li < P.n_layers; ++li) {
       // inputs of this layer (residuals, sampling sources) were written by the previous one: the producer thread polls
@@ -819,10 +719,6 @@ bool halo_layer_stages(int budget, HaloLayer& h) {
   return true;
 }
 
-bool aligned16(const void* ptr, int cstride, int coff) {
-  return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cstride % 8 == 0 && coff % 8 == 0;
-}
-
 // conv_halo_kernel's TMA epilogue for a configured fp16 layer: its tensor maps, and the stages that fit next to the
 // staging tile.  false: the layer keeps the drain epilogue (plain fp32 output, an activation without a compiled-in
 // case, 16-byte misaligned outputs or operands, a channel count that is not a multiple of 8, grouped outputs that are
@@ -843,9 +739,10 @@ bool halo_tma_configure(HaloParams& h) {
   if (p.aux0 != nullptr && !aligned16(p.aux0, p.aux0_cstride, p.aux0_coff)) return false;
   if (p.epi == PP_EPI_GRU_H && !aligned16(p.aux1, p.aux1_cstride, p.aux1_coff)) return false;
   if (p.epi == PP_EPI_GRU_ZR && !aligned16(p.out2, p.out2_cstride, p.out2_coff)) return false;
+  // the stages get what the rest of the plan leaves of SMEM_MAX
   const int region = halo_tma_region_bytes(h.MT, bn, p.epi == PP_EPI_GRU_H);
   HaloLayer staged = h;
-  if (!halo_layer_stages(SMEM_MAX - 2048 - region, staged)) return false;
+  if (!halo_layer_stages(SMEM_MAX - halo_smem(nullptr, 0, 0, 0, 0, region).bytes, staged)) return false;
   h.SA = staged.SA; h.SB = staged.SB;
   // maps: (channels, x, y, image) boxes of pw x 8 x rows / 8, or (channels, pixel) boxes of pw x rows in flat mode
   auto map = [&](CUtensorMap* m, const __half* base, int cols, int cstride) {
@@ -933,12 +830,8 @@ int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   PP_TRY(halo_set_smem_limit());
   int num_sms = 0;
   PP_TRY(pp_num_sms(&num_sms));
-  int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes;
-  if (halo_tma_configure(h)) {
-    // the TMA epilogue's region takes the place of the drain's staging tiles
-    smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes).bytes - 2 * ppconv::STG_BYTES +
-           halo_tma_region_bytes(h.MT, h.c.BN, h.c.epi == PP_EPI_GRU_H);
-  }
+  halo_tma_configure(h);   // sets h.tma_out, or the layer keeps the drain epilogue
+  const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, halo_epi_bytes(h)).bytes;
   return pp_conv_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms),
                         NUM_THREADS, smem, stream);
 }
@@ -1031,7 +924,7 @@ int pp_prog_end(unsigned int* counter, unsigned int* arrivals, cudaStream_t stre
   P.ts = (ts_mode && ts_printed < ts_mode) ? ts_dev : nullptr;
   const int grid = num_sms;
   *arrivals += (unsigned int)(P.n_layers * grid);
-  PP_TRY(pp_conv_launch(conv_prog_kernel, P, grid, NUM_THREADS, halo_smem(nullptr, sa, a_max, sb, b_max).bytes, stream));
+  PP_TRY(pp_conv_launch(conv_prog_kernel, P, grid, NUM_THREADS, halo_smem(nullptr, sa, a_max, sb, b_max, DRAIN_EPI_BYTES).bytes, stream));
   if (P.ts != nullptr) {      // debug: per-layer wall time of CTA 0 (serialises the stream)
     unsigned long long h[2 * PROG_MAX_LAYERS];
     PP_CUDA_CHECK(cudaStreamSynchronize(stream));

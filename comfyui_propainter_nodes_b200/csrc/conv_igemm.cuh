@@ -108,6 +108,12 @@ inline bool pp_conv_segs_chunked(const PPConvParams& p, bool flat) {
   return true;
 }
 
+// An fp16 pixel tensor (base pointer, elements per pixel, first channel) whose every pixel's channel run starts 16-byte
+// aligned, as TMA loads and stores of its rows need.
+inline bool aligned16(const void* ptr, int cstride, int coff) {
+  return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cstride % 8 == 0 && coff % 8 == 0;
+}
+
 // The segment that holds conv-input channel `ci`.
 __device__ __forceinline__ int pp_seg_of(const PPConvParams& p, int ci) {
   int q = 0;
