@@ -37,6 +37,8 @@ struct DeviceGuard {
   }
 
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+// null counts as aligned: optional tensors are checked only when given
+static inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // Restores the arena to its state at entry on EVERY exit of a stage call (error paths included): a failed call
 // ("workspace exhausted", bad argument after a partial allocation) must not shrink the workspace of the cached engine.
@@ -537,7 +539,6 @@ int pp_op_conv_tf32(pp_handle h, const char* name, const float* x0, int x0_C, in
 int pp_op_dcn_sample_f32(pp_handle h, const float* x0, int C0, const float* x1, int C1, const float* offs, int N,
                          int H, int W, float max_mag, float* cols, void* stream) {
   PP_HANDLE(h);
-  const auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   PP_REQUIRE(al16(x0) && al16(x1) && al16(cols), "pp_op_dcn_sample_f32: x0, x1 and cols must be 16-byte aligned");
   e.launches++;
   return pp_k_dcn_sample(x0, C0, x1, C1, offs, 432, max_mag, cols, N, H, W, as_stream(stream));
@@ -601,31 +602,154 @@ int pp_op_imgprop_step_f32(pp_handle h, const float* cur4, const float* prop_in4
 }
 
 int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,
-                    int t, int gh, int gw, int n_pool, int parity, void* stream) {
+                    const int* win_t, int n_windows, int gh, int gw, int n_pool, int parity, void* stream) {
   PP_HANDLE(h);
+  PP_REQUIRE(qkv_f16 && pkv_f16 && out_f16 && win_flags_dev && win_t && n_windows >= 1, "pp_op_attention: bad argument");
+  PP_REQUIRE(al16(qkv_f16) && al16(pkv_f16) && al16(out_f16), "pp_op_attention: qkv, pkv and out must be 16-byte aligned");
   const int nh = pp_ceil_div(gh, 5) * 5, nw = pp_ceil_div(gw, 9) * 9;
+  // the sliding windows' frames are concatenated: window w owns frames [foff[w], foff[w] + t[w]) (pp_stage_gen_run)
+  std::vector<int> meta(2 * n_windows);
+  int t_max = 0;
+  for (int w = 0, off = 0; w < n_windows; ++w) {
+    PP_REQUIRE(win_t[w] >= 2, "pp_op_attention: window %d has t=%d (< 2)", w, win_t[w]);
+    meta[w] = off;
+    meta[n_windows + w] = win_t[w];
+    off += win_t[w];
+    if (win_t[w] > t_max) t_max = win_t[w];
+  }
   std::vector<int> ring;
   pp_build_ring_indices(nh, nw, ring);
   ArenaGuard guard(e.arena);
-  int* ring_dev;
+  cudaStream_t st = as_stream(stream);
+  int *ring_dev, *meta_dev, *key_tab;
   PP_TRY(pp_alloc(e, &ring_dev, ring.size(), "ring indices"));
-  PP_CUDA_CHECK(cudaMemcpyAsync(ring_dev, ring.data(), ring.size() * sizeof(int), cudaMemcpyHostToDevice,
-                                as_stream(stream)));
+  PP_CUDA_CHECK(cudaMemcpyAsync(ring_dev, ring.data(), ring.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  PP_TRY(pp_alloc(e, &meta_dev, meta.size(), "attention meta"));
+  PP_CUDA_CHECK(cudaMemcpyAsync(meta_dev, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const int key_stride = ((t_max + 1) / 2) * (193 + n_pool);
+  PP_TRY(pp_alloc(e, &key_tab, (size_t)(nh / 5) * (nw / 9) * key_stride, "attention key table"));
   const __half* qkv = static_cast<const __half*>(qkv_f16);
   const __half* pkv = static_cast<const __half*>(pkv_f16);
-  int meta_host[2] = {0, t};
-  int* meta_dev;
-  PP_TRY(pp_alloc(e, &meta_dev, 2, "attention meta"));
-  PP_CUDA_CHECK(cudaMemcpyAsync(meta_dev, meta_host, sizeof(meta_host), cudaMemcpyHostToDevice, as_stream(stream)));
-  const int key_stride = ((t + 1) / 2) * (193 + n_pool);
-  int* key_tab;
-  PP_TRY(pp_alloc(e, &key_tab, (size_t)(nh / 5) * (nw / 9) * key_stride, "attention key table"));
-  int r = pp_k_attention(qkv, qkv + 512, qkv + 1024, 1536, pkv, pkv + 512, 1024, static_cast<__half*>(out_f16), 512,
-                         win_flags_dev, ring_dev, meta_dev, meta_dev + 1, 1, t, gh, gw, nh, nw, n_pool, parity,
-                         key_tab, key_stride, as_stream(stream));
-  PP_CUDA_CHECK(cudaStreamSynchronize(as_stream(stream)));
+  PP_TRY(pp_k_attention(qkv, qkv + 512, qkv + 1024, 1536, pkv, pkv + 512, 1024, static_cast<__half*>(out_f16), 512,
+                        win_flags_dev, ring_dev, meta_dev, meta_dev + n_windows, n_windows, t_max, gh, gw, nh, nw, n_pool,
+                        parity, key_tab, key_stride, st));
   e.launches++;
-  return r;
+  PP_CUDA_CHECK(cudaStreamSynchronize(st));   // the scratch goes back to the arena on return
+  return PP_OK;
+}
+
+int pp_op_layernorm(pp_handle h, const void* x_f16, const float* gamma, const float* beta, void* out_f16, int t, int gh,
+                    int gw, int nh, int nw, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(x_f16 && gamma && beta && out_f16, "pp_op_layernorm: null pointer");
+  PP_REQUIRE(al16(x_f16) && al16(gamma) && al16(beta) && al16(out_f16),
+             "pp_op_layernorm: x, gamma, beta and out must be 16-byte aligned");
+  PP_REQUIRE(t >= 0 && gh >= 1 && gw >= 1 && nh >= gh && nw >= gw, "pp_op_layernorm: grid %dx%d in %dx%d", gh, gw, nh, nw);
+  e.launches++;
+  return pp_k_layernorm(static_cast<const __half*>(x_f16), gamma, beta, static_cast<__half*>(out_f16),
+                        (long long)t * gh * gw, gh, gw, nh, nw, as_stream(stream));
+}
+
+int pp_op_pool_tokens(pp_handle h, const void* x_f16, const float* w, const float* b, void* out_f16, int t, int nh,
+                      int nw, int C, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(x_f16 && w && b && out_f16, "pp_op_pool_tokens: null pointer");
+  PP_REQUIRE(al16(x_f16) && al16(w) && al16(b) && al16(out_f16), "pp_op_pool_tokens: x, w, b and out must be 16-byte aligned");
+  PP_REQUIRE(nh >= 4 && nw >= 4, "pp_op_pool_tokens: grid %dx%d is smaller than the 4x4 pooling window", nh, nw);
+  e.launches++;
+  return pp_k_pool_tokens(static_cast<const __half*>(x_f16), w, b, static_cast<__half*>(out_f16), t, nh, nw,
+                          (nh - 4) / 4 + 1, (nw - 4) / 4 + 1, C, as_stream(stream));
+}
+
+int pp_op_window_flags(pp_handle h, const void* mask4_f16, int cs, int co, const int* win_f0, const int* win_lt,
+                       int n_windows, int h4, int w4, int* flags_dev, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(mask4_f16 && win_f0 && win_lt && flags_dev && n_windows >= 1 && h4 >= 1 && w4 >= 1 && co < cs,
+             "pp_op_window_flags: bad argument");
+  const int gh = (h4 - 1) / 3 + 1, gw = (w4 - 1) / 3 + 1;   // unfold(7, stride 3, pad 3) token grid
+  std::vector<int> meta(win_f0, win_f0 + n_windows);
+  meta.insert(meta.end(), win_lt, win_lt + n_windows);
+  ArenaGuard guard(e.arena);
+  cudaStream_t st = as_stream(stream);
+  int* meta_dev;
+  PP_TRY(pp_alloc(e, &meta_dev, meta.size(), "window flag meta"));
+  PP_CUDA_CHECK(cudaMemcpyAsync(meta_dev, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  PP_TRY(pp_k_window_flags(static_cast<const __half*>(mask4_f16), cs, co, meta_dev, meta_dev + n_windows, n_windows, h4,
+                           w4, gh, gw, pp_ceil_div(gh, 5), pp_ceil_div(gw, 9), flags_dev, st));
+  e.launches++;
+  PP_CUDA_CHECK(cudaStreamSynchronize(st));
+  return PP_OK;
+}
+
+int pp_op_fold(pp_handle h, const void* x_f16, int cs, void* out_f16, int t, int H, int W, int C, int normalise, int gelu,
+               void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(x_f16 && out_f16 && H >= 1 && W >= 1 && C <= cs / 49, "pp_op_fold: bad argument (C=%d cs=%d)", C, cs);
+  PP_REQUIRE(al16(x_f16) && al16(out_f16), "pp_op_fold: x and out must be 16-byte aligned");
+  e.launches++;
+  return pp_k_fold(static_cast<const __half*>(x_f16), cs, static_cast<__half*>(out_f16), t, H, W, C, (H - 1) / 3 + 1,
+                   (W - 1) / 3 + 1, normalise, gelu, as_stream(stream));
+}
+
+int pp_op_featprop_cond(pp_handle h, const void* cur_f16, const void* prop_f16, const void* flow_prop_f16,
+                        const void* flow_check_f16, const void* mask2_f16, void* cond_f16, int N, int H, int W,
+                        void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(cur_f16 && prop_f16 && flow_prop_f16 && flow_check_f16 && mask2_f16 && cond_f16,
+             "pp_op_featprop_cond: null pointer");
+  PP_REQUIRE(al16(cur_f16) && al16(prop_f16) && al16(mask2_f16) && al16(cond_f16) &&
+                 ((reinterpret_cast<uintptr_t>(flow_prop_f16) | reinterpret_cast<uintptr_t>(flow_check_f16)) & 3) == 0,
+             "pp_op_featprop_cond: cur, prop, mask2 and cond must be 16-byte aligned, the flows 4-byte aligned");
+  e.launches++;
+  return pp_k_featprop_cond(static_cast<const __half*>(cur_f16), 128, static_cast<const __half*>(prop_f16), 128,
+                            static_cast<const __half*>(flow_prop_f16), static_cast<const __half*>(flow_check_f16),
+                            static_cast<const __half*>(mask2_f16), 8, static_cast<__half*>(cond_f16), 264, N, H, W, 128,
+                            as_stream(stream));
+}
+
+int pp_op_dcn_sample(pp_handle h, const void* x0_f16, int x0_cs, int C0, const void* x1_f16, int x1_cs, int C1,
+                     const void* offs_f16, const void* flow_f16, int flow_cs, int flow_co, float max_mag, void* cols_f16,
+                     int N, int H, int W, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(x0_f16 && offs_f16 && cols_f16 && (C1 == 0 || x1_f16), "pp_op_dcn_sample: null pointer");
+  PP_REQUIRE(al16(x0_f16) && al16(x1_f16) && al16(cols_f16) && x0_cs % 8 == 0 && (C1 == 0 || x1_cs % 8 == 0),
+             "pp_op_dcn_sample: x0, x1 and cols must be 16-byte aligned with channel strides that are multiples of 8");
+  PP_REQUIRE(C0 <= x0_cs && (C1 == 0 || C1 <= x1_cs), "pp_op_dcn_sample: channels exceed the channel strides");
+  PP_REQUIRE(flow_f16 == nullptr || flow_co + 2 <= flow_cs, "pp_op_dcn_sample: flow channels %d..%d of %d", flow_co,
+             flow_co + 1, flow_cs);
+  e.launches++;
+  return pp_k_dcn_sample(static_cast<const __half*>(x0_f16), x0_cs, 0, C0, static_cast<const __half*>(x1_f16), x1_cs, 0,
+                         C1, static_cast<const __half*>(offs_f16), 432, static_cast<const __half*>(flow_f16), flow_cs,
+                         flow_co, max_mag, static_cast<__half*>(cols_f16), N, H, W, as_stream(stream));
+}
+
+int pp_op_downsample4(pp_handle h, const float* flows, void* flows4_f16, int n_flows, const float* masks,
+                      void* masks4_f16, int mask_co, int n_masks, int H, int W, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE((flows == nullptr) == (flows4_f16 == nullptr) && (masks == nullptr) == (masks4_f16 == nullptr) &&
+                 mask_co >= 0 && mask_co < 8,
+             "pp_op_downsample4: bad argument");
+  PP_REQUIRE(H % 4 == 0 && W % 4 == 0, "pp_op_downsample4: size %dx%d must be a multiple of 4", W, H);
+  PP_REQUIRE((reinterpret_cast<uintptr_t>(flows4_f16) & 3) == 0, "pp_op_downsample4: flows4 must be 4-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  if (flows != nullptr) {
+    PP_TRY(pp_k_downsample_flow4(flows, static_cast<__half*>(flows4_f16), n_flows, H, W, st));
+    e.launches++;
+  }
+  if (masks != nullptr) {
+    PP_TRY(pp_k_downsample_mask4(masks, static_cast<__half*>(masks4_f16), 8, mask_co, n_masks, H, W, st));
+    e.launches++;
+  }
+  return PP_OK;
+}
+
+int pp_op_upsample2x(pp_handle h, const void* src_f16, void* dst_f16, int N, int H, int W, int C, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(src_f16 && dst_f16, "pp_op_upsample2x: null pointer");
+  PP_REQUIRE(al16(src_f16) && al16(dst_f16), "pp_op_upsample2x: src and dst must be 16-byte aligned");
+  e.launches++;
+  return pp_k_upsample2x(static_cast<const __half*>(src_f16), C, 0, static_cast<__half*>(dst_f16), C, 0, N, H, W, C,
+                         as_stream(stream));
 }
 
 }  // extern "C"

@@ -188,6 +188,9 @@ int pp_stage_gen_run(PPEngine& e, const int* frame_ids, const int* win_t, const 
   for (int w = 0; w < n_sw; ++w) {
     const int t = win_t[w], lt = win_lt[w];
     PP_REQUIRE(lt >= 1 && lt <= t, "generator: window %d has l_t=%d t=%d", w, lt, t);
+    // the odd transformer blocks attend to frames 1, 3, ...: a window of one frame leaves its masked 5x9 windows
+    // without keys there
+    PP_REQUIRE(t >= 2, "generator: window %d has t=%d frames; a window needs at least 2", w, t);
     const int* ids = frame_ids + foff[w];
     for (int i = 0; i < t; ++i) PP_REQUIRE(ids[i] >= 0 && ids[i] < g.T, "generator: frame id out of range");
     for (int i = 1; i < lt; ++i) PP_REQUIRE(ids[i] == ids[0] + i, "generator: local frames must be consecutive");

@@ -33,22 +33,27 @@ __global__ void __launch_bounds__(256) layernorm512(const __half* __restrict__ x
     uint4 raw[2] = {xp[0], xp[1]};
     float v[16];
     const __half2* h = reinterpret_cast<const __half2*>(raw);
-    float s = 0.f, q = 0.f;
+    float s = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const float2 f = __half22float2(h[i]);
       v[2 * i] = f.x; v[2 * i + 1] = f.y;
       s += f.x + f.y;
-      q += f.x * f.x + f.y * f.y;
     }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      s += __shfl_xor_sync(0xffffffffu, s, o);
-      q += __shfl_xor_sync(0xffffffffu, q, o);
-    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     const float mean = s * (1.f / 512.f);
-    const float var = fmaxf(q * (1.f / 512.f) - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + 1e-5f);
+    // two-pass variance over the values already in registers: E[x^2] - mean^2 cancels catastrophically once
+    // |mean| / std reaches ~30 (fp32 sums of x^2 lose the variance in their rounding)
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float a = v[2 * i] - mean, b = v[2 * i + 1] - mean;
+      q += a * a + b * b;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    const float rstd = rsqrtf(q * (1.f / 512.f) + 1e-5f);
     __align__(16) __half2 o2[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i)

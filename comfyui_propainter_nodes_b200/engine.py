@@ -75,7 +75,15 @@ _SIGNATURES = {
     "pp_op_convex_upsample": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "pp_op_imgprop_step": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP]),
     "pp_op_imgprop_step_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _VP]),
-    "pp_op_attention": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "pp_op_attention": (_I, [_VP, _VP, _VP, _VP, _VP, ctypes.POINTER(_I), _I, _I, _I, _I, _I, _VP]),
+    "pp_op_layernorm": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "pp_op_pool_tokens": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
+    "pp_op_window_flags": (_I, [_VP, _VP, _I, _I, ctypes.POINTER(_I), ctypes.POINTER(_I), _I, _I, _I, _VP, _VP]),
+    "pp_op_fold": (_I, [_VP, _VP, _I, _VP, _I, _I, _I, _I, _I, _I, _VP]),
+    "pp_op_featprop_cond": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
+    "pp_op_dcn_sample": (_I, [_VP, _VP, _I, _I, _VP, _I, _I, _VP, _VP, _I, _I, _F, _VP, _I, _I, _I, _VP]),
+    "pp_op_downsample4": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _I, _I, _I, _I, _VP]),
+    "pp_op_upsample2x": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP]),
 }
 
 
@@ -884,8 +892,87 @@ class Engine:
                                                     _ptr(flow_check), H, W, self._stream()))
         return out
 
-    def op_attention(self, qkv, pkv, win_flags, t, gh, gw, n_pool, parity):
-        out = torch.zeros(t, gh, gw, 512, device=self.device, dtype=torch.float16)
-        self._check(self.lib.pp_op_attention(self.h, _ptr(qkv), _ptr(pkv), _ptr(out), _ptr(win_flags), t, gh, gw, n_pool,
-                                             parity, self._stream()))
+    def op_attention(self, qkv, pkv, win_flags, win_t, gh, gw, n_pool, parity):
+        """Sparse window attention of sliding windows with win_t[w] frames each, concatenated: qkv fp16
+        [sum(win_t), nh*nw, 1536], pkv fp16 [sum(win_t), n_pool, 1024], win_flags int32 [len(win_t), nwh*nww]
+        -> [sum(win_t), gh, gw, 512].  An int win_t is one sliding window of that many frames."""
+        win_t = [int(win_t)] if isinstance(win_t, int) else [int(t) for t in win_t]
+        out = torch.zeros(sum(win_t), gh, gw, 512, device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_attention(self.h, _ptr(qkv), _ptr(pkv), _ptr(out), _ptr(win_flags),
+                                             (ctypes.c_int * len(win_t))(*win_t), len(win_t), gh, gw, n_pool, parity,
+                                             self._stream()))
+        return out
+
+    def op_layernorm(self, x, gamma, beta, gh, gw, nh, nw, fill=0.0):
+        """LayerNorm(512) of x fp16 [t*gh*gw, 512] -> fp16 [t, nh, nw, 512]; padding rows keep `fill`."""
+        t = x.shape[0] // (gh * gw)
+        out = torch.full((t, nh, nw, 512), fill, device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_layernorm(self.h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), t, gh, gw, nh, nw,
+                                             self._stream()))
+        return out
+
+    def op_pool_tokens(self, x, w, b):
+        """Depthwise 4x4 stride-4 pooling of x fp16 [t, nh, nw, C], w float32 [16, C] (tap-major), b float32 [C]."""
+        t, nh, nw, C = x.shape
+        out = torch.empty(t, (nh - 4) // 4 + 1, (nw - 4) // 4 + 1, C, device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_pool_tokens(self.h, _ptr(x), _ptr(w), _ptr(b), _ptr(out), t, nh, nw, C,
+                                               self._stream()))
+        return out
+
+    def op_window_flags(self, mask4, co, win_f0, win_lt):
+        """mask4 fp16 [T, h4, w4, cs] (channel co) -> int32 [len(win_f0), nwh*nww] masked-window flags."""
+        _, h4, w4, cs = mask4.shape
+        gh, gw = (h4 - 1) // 3 + 1, (w4 - 1) // 3 + 1
+        n = len(win_f0)
+        flags = torch.full((n, -(-gh // 5) * -(-gw // 9)), -1, device=self.device, dtype=torch.int32)
+        arr = lambda v: (ctypes.c_int * n)(*[int(i) for i in v])
+        self._check(self.lib.pp_op_window_flags(self.h, _ptr(mask4), cs, co, arr(win_f0), arr(win_lt), n, h4, w4,
+                                                _ptr(flags), self._stream()))
+        return flags
+
+    def op_fold(self, x, t, H, W, C, normalise, gelu):
+        """F.fold(7, stride 3, pad 3) of x fp16 [t*gh*gw, cs] -> fp16 [t, H, W, C]."""
+        out = torch.empty(t, H, W, C, device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_fold(self.h, _ptr(x), x.shape[-1], _ptr(out), t, H, W, C, int(normalise), int(gelu),
+                                        self._stream()))
+        return out
+
+    def op_featprop_cond(self, cur, prop, flow_prop, flow_check, mask2):
+        """cur / prop fp16 [N, H, W, 128], flows fp16 [N, H, W, 2], mask2 fp16 [N, H, W, 8] -> cond fp16 [N, H, W, 264]."""
+        N, H, W, _ = cur.shape
+        cond = torch.full((N, H, W, 264), float("nan"), device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_featprop_cond(self.h, _ptr(cur), _ptr(prop), _ptr(flow_prop), _ptr(flow_check),
+                                                 _ptr(mask2), _ptr(cond), N, H, W, self._stream()))
+        return cond
+
+    def op_dcn_sample(self, x0, offs, max_mag, x1=None, flow=None):
+        """fp16 deformable sampler: x0 [N, H, W, C0] (+ x1 [N, H, W, C1]), offs [N, H, W, 432], flow = (tensor
+        [N, H, W, cs], co) or None -> columns fp16 [N, H, W, 9 * (C0 + C1)]."""
+        N, H, W, C0 = x0.shape
+        C1 = 0 if x1 is None else x1.shape[-1]
+        ft, fco = flow if flow is not None else (None, 0)
+        cols = torch.empty(N, H, W, 9 * (C0 + C1), device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_dcn_sample(self.h, _ptr(x0), C0, C0, _ptr(x1), C1, C1, _ptr(offs), _ptr(ft),
+                                              0 if ft is None else ft.shape[-1], fco, float(max_mag), _ptr(cols), N, H,
+                                              W, self._stream()))
+        return cols
+
+    def op_downsample4(self, flows=None, masks=None, mask_co=0):
+        """flows float32 [n, 2, H, W] -> fp16 [n, H/4, W/4, 2]; masks float32 [n, 1, H, W] -> fp16 [n, H/4, W/4, 8]
+        (channel mask_co written, the others zero)."""
+        H, W = (flows if flows is not None else masks).shape[-2:]
+        f4 = None if flows is None else torch.empty(flows.shape[0], H // 4, W // 4, 2, device=self.device,
+                                                    dtype=torch.float16)
+        m4 = None if masks is None else torch.zeros(masks.shape[0], H // 4, W // 4, 8, device=self.device,
+                                                    dtype=torch.float16)
+        self._check(self.lib.pp_op_downsample4(self.h, _ptr(flows), _ptr(f4), 0 if flows is None else flows.shape[0],
+                                               _ptr(masks), _ptr(m4), mask_co, 0 if masks is None else masks.shape[0],
+                                               H, W, self._stream()))
+        return f4, m4
+
+    def op_upsample2x(self, x):
+        """bilinear x2 (align_corners=True) of fp16 [N, H, W, C] -> [N, 2H, 2W, C]."""
+        N, H, W, C = x.shape
+        out = torch.empty(N, 2 * H, 2 * W, C, device=self.device, dtype=torch.float16)
+        self._check(self.lib.pp_op_upsample2x(self.h, _ptr(x), _ptr(out), N, H, W, C, self._stream()))
         return out

@@ -273,8 +273,13 @@ def synthetic_rfc_state_dict(seed: int = 1):
     return _fill(rfc_spec(), seed, gain)
 
 
-def synthetic_generator_state_dict(seed: int = 2):
+def synthetic_generator_state_dict(seed: int = 2, attn_logit_gain: float = 1.0):
+    """Seeded generator checkpoint.  ``attn_logit_gain`` scales the attention's query and key weights, so the logits by
+    its square: at 1.0 (default, the bench weights) the attention over ~1,600 keys is nearly uniform; a larger gain makes
+    it sharp, so that a key gathered from the wrong token moves the output by O(|v|)."""
     def gain(key, shape):
+        if "attention.query.weight" in key or "attention.key.weight" in key:
+            return attn_logit_gain
         if "backbone" in key and key.endswith(".2.weight"):
             return 0.3
         if "conv_offset.6" in key:

@@ -223,8 +223,47 @@ PP_API int pp_op_imgprop_step(pp_handle h, const void* cur4_f16, const void* pro
  * [H][W][2]. */
 PP_API int pp_op_imgprop_step_f32(pp_handle h, const float* cur4, const float* prop_in4, float* prop_out4,
                                   const float* flow_prop, const float* flow_check, int H, int W, void* stream);
+/* Operators of the generator (pp_gen_run), fp16 NHWC, each one launch of the kernel the stage runs.  Token grids: gh x gw
+ * tokens of a frame (unfold 7x7, stride 3, pad 3 of an h4 x w4 feature map), padded to nh x nw (multiples of 5 x 9).
+ * Sparse window attention of sliding windows whose frames are concatenated (window w owns win_t[w] >= 2 frames, host
+ * array): qkv [frames][nh*nw][q 512 | k 512 | v 512], pooled pkv [frames][n_pool][k 512 | v 512] -> out [frames][gh][gw][512];
+ * win_flags_dev [n_windows][(nh/5)*(nw/9)] (device) selects the masked 5x9 windows; key frames are parity, parity+2, ... */
 PP_API int pp_op_attention(pp_handle h, const void* qkv_f16, const void* pkv_f16, void* out_f16, const int* win_flags_dev,
-                    int t, int gh, int gw, int n_pool, int parity, void* stream);
+                           const int* win_t, int n_windows, int gh, int gw, int n_pool, int parity, void* stream);
+/* LayerNorm over 512 channels (eps 1e-5, fp32 gamma / beta): x [t*gh*gw][512] -> out [t][nh][nw][512]; rows of the
+ * padding are not written. */
+PP_API int pp_op_layernorm(pp_handle h, const void* x_f16, const float* gamma, const float* beta, void* out_f16, int t,
+                           int gh, int gw, int nh, int nw, void* stream);
+/* Depthwise 4x4 stride-4 pooling: x [t][nh][nw][C], w fp32 [16 taps][C], b fp32 [C] -> out [t][ph][pw][C] with
+ * ph = (nh - 4) / 4 + 1, pw = (nw - 4) / 4 + 1. */
+PP_API int pp_op_pool_tokens(pp_handle h, const void* x_f16, const float* w, const float* b, void* out_f16, int t, int nh,
+                             int nw, int C, void* stream);
+/* Masked-window flags: mask4 [frames][h4][w4][cs] (channel co), sliding window w covers frames win_f0[w] ..
+ * win_f0[w] + win_lt[w] - 1 (host arrays) -> flags_dev [n_windows][(nh/5)*(nw/9)] (device int32). */
+PP_API int pp_op_window_flags(pp_handle h, const void* mask4_f16, int cs, int co, const int* win_f0, const int* win_lt,
+                              int n_windows, int h4, int w4, int* flags_dev, void* stream);
+/* F.fold(7x7, stride 3, pad 3) of x [t*gh*gw][cs] (column (ky*7 + kx)*C + c) -> out [t][H][W][C]; gh / gw derived from
+ * H / W; normalise divides by the overlap count, gelu applies erf-GELU after it. */
+PP_API int pp_op_fold(pp_handle h, const void* x_f16, int cs, void* out_f16, int t, int H, int W, int C, int normalise,
+                      int gelu, void* stream);
+/* DCN condition of one feature-propagation step: cur / prop [N][H][W][128], flows [N][H][W][2], mask2 [N][H][W][8] ->
+ * cond [N][H][W][264] = (cur 128 | prop warped by flow_prop 128 | flow_prop 2 | fb validity 1 | mask2[0..1] 2 | 0 0 0). */
+PP_API int pp_op_featprop_cond(pp_handle h, const void* cur_f16, const void* prop_f16, const void* flow_prop_f16,
+                               const void* flow_check_f16, const void* mask2_f16, void* cond_f16, int N, int H, int W,
+                               void* stream);
+/* fp16 modulated deformable sampling (3x3, pad 1, 16 offset groups of (C0 + C1) / 16 channels, C0 + C1 = 128 or 256):
+ * x0 [pix][x0_cs] channels 0..C0-1, x1 [pix][x1_cs] channels 0..C1-1 (x1 may be NULL when C1 = 0), offs [pix][432];
+ * offsets max_mag * tanh, plus, with flow not NULL, the flow (x at channel flow_co, y at flow_co + 1 of [pix][flow_cs]);
+ * -> cols [pix][9 * (C0 + C1)] ordered (tap, channel). */
+PP_API int pp_op_dcn_sample(pp_handle h, const void* x0_f16, int x0_cs, int C0, const void* x1_f16, int x1_cs, int C1,
+                            const void* offs_f16, const void* flow_f16, int flow_cs, int flow_co, float max_mag,
+                            void* cols_f16, int N, int H, int W, void* stream);
+/* 1/4 downsampling of pp_gen_begin: flows fp32 [n_flows][2][H][W] -> bilinear / 4 [n_flows][H/4][W/4][2]; masks fp32
+ * [n_masks][1][H][W] -> nearest, channel mask_co of [n_masks][H/4][W/4][8].  Either pair may be NULL. */
+PP_API int pp_op_downsample4(pp_handle h, const float* flows, void* flows4_f16, int n_flows, const float* masks,
+                             void* masks4_f16, int mask_co, int n_masks, int H, int W, void* stream);
+/* Bilinear x2 upsampling (align_corners=True): src [N][H][W][C] -> dst [N][2H][2W][C] (C a multiple of 8). */
+PP_API int pp_op_upsample2x(pp_handle h, const void* src_f16, void* dst_f16, int N, int H, int W, int C, void* stream);
 
 #ifdef __cplusplus
 }

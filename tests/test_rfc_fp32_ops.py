@@ -21,25 +21,24 @@ pytestmark = pytest.mark.gpu
 
 
 # ------------------------------------------------------------------------------------------------ references
-def im2col_reference(x, offs, dtype, max_mag=5.0, tanh=torch.tanh, lo=True):
+def im2col_reference(x, offs, dtype, max_mag=5.0, tanh=torch.tanh, lo=True, flow=None, sigmoid=torch.sigmoid,
+                     pos_delta=0.0):
     """torchvision's modulated deformable im2col (3x3, pad 1, 16 offset groups) in `dtype` on the CPU.
     x [N,H,W,C], offs [N,H,W,432] (offsets (g*9+k)*2 + {0: dy, 1: dx} before max_mag*tanh, modulation 288 + g*9+k
     before the sigmoid) -> columns [N,H,W,9*C] ordered (tap, channel).  lo=False emulates columns without their lo part
-    (tf32-rounded)."""
+    (tf32-rounded).  flow [N,H,W,2] (x, y) is added to every offset (the generator's DeformableAlignment:
+    offset + flow.flip(1)).  pos_delta > 0 also returns the largest change of each column when its sample position
+    moves by up to pos_delta px in y and x: bilinear interpolation is bilinear inside a cell of the pixel grid, so that
+    maximum is attained at a corner of the box, where the box crosses a grid line, or where two grid lines cross."""
     N, H, W, C = x.shape
     x, o = x.to(dtype), offs.to(dtype)
     cpg = C // 16
     ys = torch.arange(H, dtype=dtype).view(1, H, 1, 1)
     xs = torch.arange(W, dtype=dtype).view(1, 1, W, 1)
     flat = x.reshape(N, H * W, C)
-    cols = torch.zeros(N, H, W, 9, C, dtype=dtype)
-    for k in range(9):
-        gk = torch.arange(16) * 9 + k
-        dy = max_mag * tanh(o[..., 2 * gk])
-        dx = max_mag * tanh(o[..., 2 * gk + 1])
-        mod = torch.sigmoid(o[..., 288 + gk])
-        py = (ys + (k // 3 - 1)) + dy                                  # [N,H,W,16]
-        px = (xs + (k % 3 - 1)) + dx
+    ch = torch.arange(C).view(16, cpg)
+
+    def sample(py, px):                                                # [N,H,W,16] positions -> [N,H,W,16,cpg]
         inside = (py > -1) & (py < H) & (px > -1) & (px < W)
         y0, x0 = torch.floor(py), torch.floor(px)
         lh, lw = py - y0, px - x0
@@ -48,14 +47,38 @@ def im2col_reference(x, offs, dtype, max_mag=5.0, tanh=torch.tanh, lo=True):
         for wgt, yy, xx in ((hh * hw, y0, x0), (hh * lw, y0, x0 + 1), (lh * hw, y0 + 1, x0), (lh * lw, y0 + 1, x0 + 1)):
             ok = inside & (yy >= 0) & (yy < H) & (xx >= 0) & (xx < W)
             idx = (yy.clamp(0, H - 1) * W + xx.clamp(0, W - 1)).long()   # [N,H,W,16]
-            ch = torch.arange(C).view(16, cpg)
             g = flat[torch.arange(N).view(N, 1, 1, 1, 1), idx.unsqueeze(-1), ch.view(1, 1, 1, 16, cpg)]
             val = val + (wgt * ok).unsqueeze(-1) * g
-        cols[:, :, :, k] = (mod.unsqueeze(-1) * val).reshape(N, H, W, C)
+        return val
+
+    def box(p):                                                        # box edges and the grid line inside, if any
+        r = torch.round(p)
+        return (p - pos_delta, p + pos_delta, torch.where((r - p).abs() < pos_delta, r, p))
+
+    cols = torch.zeros(N, H, W, 9, C, dtype=dtype)
+    dev = torch.zeros(N, H, W, 9, C, dtype=dtype)
+    for k in range(9):
+        gk = torch.arange(16) * 9 + k
+        dy = max_mag * tanh(o[..., 2 * gk])
+        dx = max_mag * tanh(o[..., 2 * gk + 1])
+        if flow is not None:
+            dy = dy + flow[..., 1:2].to(dtype)
+            dx = dx + flow[..., 0:1].to(dtype)
+        mod = sigmoid(o[..., 288 + gk]).unsqueeze(-1)
+        py = (ys + (k // 3 - 1)) + dy                                  # [N,H,W,16]
+        px = (xs + (k % 3 - 1)) + dx
+        val = sample(py, px)
+        cols[:, :, :, k] = (mod * val).reshape(N, H, W, C)
+        if pos_delta > 0:
+            d = torch.zeros_like(val)
+            for qy in box(py):
+                for qx in box(px):
+                    d = torch.maximum(d, (sample(qy, qx) - val).abs())
+            dev[:, :, :, k] = (mod * d).reshape(N, H, W, C)
     cols = cols.reshape(N, H, W, 9 * C)
     if not lo:
         cols = E.split_tf32(cols.float())[0].to(dtype)
-    return cols
+    return (cols, dev.reshape(N, H, W, 9 * C)) if pos_delta > 0 else cols
 
 
 def sampler_case(seed, H=23, W=37, N=2):
