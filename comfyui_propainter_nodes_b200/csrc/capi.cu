@@ -503,6 +503,42 @@ int pp_op_conv_ex(pp_handle h, const char* name, const void* x_f16, int x_C, int
   return c.run(as_stream(stream));
 }
 
+int pp_op_conv_segs(pp_handle h, const char* name, int nseg, const void* const* x_f16, const int* x_C, const int* x_co,
+                    const int* x_ch, const int* x_gstep, int N, int H, int W, int sh, int sw, int ph, int pw, int dh,
+                    int dw, int replicate, int epi, int act, float slope, float scale, int act2, const void* aux0_f16,
+                    int aux0_C, int aux0_co, void* aux1_f16, int aux1_C, int aux1_co, void* out, int out_C, int out_co,
+                    int out_gstep, int out_fp32, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(name && x_f16 && x_C && x_co && x_ch && x_gstep && out, "pp_op_conv_segs: null pointer");
+  PP_REQUIRE(nseg >= 1 && nseg <= PP_MAX_SEGS, "pp_op_conv_segs: %d input segments (1..%d)", nseg, PP_MAX_SEGS);
+  PP_REQUIRE(epi == PP_EPI_STD || (aux0_f16 && aux1_f16 && !out_fp32),
+             "pp_op_conv_segs: the GRU epilogues need aux0 and aux1 and an fp16 output");
+  PPConvCall c(e, name, N, H, W);
+  for (int i = 0; i < nseg; ++i) c.in(static_cast<const __half*>(x_f16[i]), x_C[i], x_co[i], x_ch[i], x_gstep[i]);
+  c.geom(sh, sw, ph, pw, dh, dw, replicate);
+  if (out_fp32) c.out_f32(static_cast<float*>(out), out_C, out_co);
+  else c.out(static_cast<__half*>(out), out_C, out_co, out_gstep);
+  const __half* a0 = static_cast<const __half*>(aux0_f16);
+  __half* a1 = static_cast<__half*>(aux1_f16);
+  if (epi == PP_EPI_GRU_ZR) {
+    c.gru_zr(a0, aux0_C, aux0_co, a1, aux1_C, aux1_co);
+  } else if (epi == PP_EPI_GRU_H) {
+    c.gru_h(a0, aux0_C, aux0_co, a1, aux1_C, aux1_co);
+  } else {
+    c.act(act, slope, scale, act2);
+    if (a0 != nullptr) c.residual(a0, aux0_C, aux0_co);
+  }
+  return c.run(as_stream(stream));
+}
+
+int pp_op_conv_last_plan(int* plan, int n) {
+  PP_REQUIRE(plan != nullptr && n >= 0, "pp_op_conv_last_plan: bad argument");
+  const PPConvPlan& p = pp_last_conv_plan();
+  const int v[8] = {p.kind, p.m, p.bn, p.tps, p.flat, p.tma_out, p.sa, p.sb};
+  for (int i = 0; i < n && i < 8; ++i) plan[i] = v[i];
+  return PP_OK;
+}
+
 int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream) {
   PP_HANDLE(h);

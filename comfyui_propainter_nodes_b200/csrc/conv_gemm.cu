@@ -209,6 +209,10 @@ int pp_conv_gemm_eligible(const PPConvParams& p) {
   if (!pp_conv_segs_chunked(p, true)) return 0;
   // TMA stores (and residual loads): 16-byte aligned rows
   if (!aligned16(p.out, p.out_cstride, p.out_coff)) return 0;
+  // TMA stores clip the channel dimension at 16-byte granularity (measured on H100: layers of 2, 10 and 126 channels
+  // written into a wider tensor overwrote the channels up to the next multiple of 8), so a channel count that ends
+  // inside a 16-byte unit would overwrite its neighbours; such layers run on the halo kernel's drain epilogue
+  if (p.Cout_g % 8 != 0) return 0;
   if (p.aux0 != nullptr && !aligned16(p.aux0, p.aux0_cstride, p.aux0_coff)) return 0;
   if (p.bias != nullptr && (reinterpret_cast<uintptr_t>(p.bias) & 7) != 0) return 0;
   // launches of less than one wave keep the halo kernel, which narrows its tiles to fill the SMs
@@ -240,6 +244,7 @@ int pp_launch_conv_gemm(const PPConvParams& pin, cudaStream_t stream) {
     PP_TRY(pp_tmap_2d_f16(&h.tmap_res, p.aux0 + p.aux0_coff, p.Cout_g, p.M_total, p.aux0_cstride, 64 * mb));
   int num_sms = 0;
   PP_TRY(pp_num_sms(&num_sms));
+  pp_last_conv_plan() = PPConvPlan{'g', mb, 256 / mb, 0, 1, 1, STAGES, STAGES};
   return pp_conv_launch(mb == 2 ? conv_gemm_kernel<2> : conv_gemm_kernel<1>, h, min(h.m_tiles * h.n_tiles, num_sms),
                         NUM_THREADS, SMEM_BYTES, stream);
 }

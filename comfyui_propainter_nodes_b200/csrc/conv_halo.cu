@@ -831,6 +831,7 @@ int pp_launch_conv_halo(const PPConvParams& pin, cudaStream_t stream) {
   int num_sms = 0;
   PP_TRY(pp_num_sms(&num_sms));
   halo_tma_configure(h);   // sets h.tma_out, or the layer keeps the drain epilogue
+  pp_last_conv_plan() = PPConvPlan{'h', h.MT, h.c.BN, h.tps, h.flat, h.tma_out, h.SA, h.SB};
   const int smem = halo_smem(nullptr, h.SA, h.a_stage_bytes, h.SB, h.b_stage_bytes, halo_epi_bytes(h)).bytes;
   return pp_conv_launch(h.c.split ? conv_halo_tf32_kernel : conv_halo_kernel, h, min(halo_total_tiles(h), num_sms),
                         NUM_THREADS, smem, stream);

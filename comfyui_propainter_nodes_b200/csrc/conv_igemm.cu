@@ -206,9 +206,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_igemm_tf32_kernel(const _
 }  // namespace
 
 namespace {
-thread_local char g_last_kind = '?';
+thread_local PPConvPlan g_last_plan = {'?', 0, 0, 0, 0, 0, 0, 0};
 }
-char pp_last_conv_kind() { return g_last_kind; }
+PPConvPlan& pp_last_conv_plan() { return g_last_plan; }
 
 int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   PPConvParams p = pin;
@@ -250,14 +250,14 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
     if (p.epi == PP_EPI_GRU_ZR) ok = ok && ((p.Cout_g >> 1) % 16 == 0);
     p.vec_ok = ok ? 1 : 0;
   }
+  g_last_plan = PPConvPlan{'?', 0, 0, 0, 0, 0, 0, 0};
   if (pp_prog_recording()) {
     PP_REQUIRE(!p.split, "conv program: split-tf32 layers are not supported");
-    g_last_kind = 'p';
+    g_last_plan.kind = 'p';
     return pp_prog_record_conv(p);
   }
-  if (pp_conv_gemm_eligible(p)) { g_last_kind = 'g'; return pp_launch_conv_gemm(p, stream); }
-  if (pp_conv_halo_eligible(p)) { g_last_kind = 'h'; return pp_launch_conv_halo(p, stream); }
-  g_last_kind = 'i';
+  if (pp_conv_gemm_eligible(p)) return pp_launch_conv_gemm(p, stream);   // both launchers record their plan
+  if (pp_conv_halo_eligible(p)) return pp_launch_conv_halo(p, stream);
   for (int i = 0; i < p.nseg; ++i)
     PP_REQUIRE(p.seg[i].cvalid == 0, "conv: zero-extended input channels (cvalid=%d of %d) need the TMA halo kernel "
                "(stride 1, zero padding, Cin %% 64 == 0)", p.seg[i].cvalid, p.seg[i].cend - p.seg[i].cbegin);   // stride-1 k>1 layers: TMA halo-tile kernel
@@ -265,6 +265,7 @@ int pp_launch_conv(const PPConvParams& pin, cudaStream_t stream) {
   int stages = SMEM_BUDGET / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   p.stages = stages;
+  g_last_plan = PPConvPlan{'i', 0, p.BN, 0, 0, 0, stages, stages};
   const size_t smem = (size_t)stages * stage_bytes + 2 * ppconv::STG_BYTES + 1024 + 256;
   static bool smem_limit_set = false;
   if (!smem_limit_set) {

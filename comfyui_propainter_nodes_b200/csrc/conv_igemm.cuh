@@ -69,9 +69,22 @@ struct PPConvParams {
 };
 
 int pp_launch_conv(const PPConvParams& p, cudaStream_t stream);
-// which kernel the last pp_launch_conv of this thread went to: 'g' flat GEMM kernel, 'h' TMA halo-tile kernel,
-// 'i' cp.async implicit GEMM, 'p' recorded into a multi-layer program (profiling labels)
-char pp_last_conv_kind();
+// The tile plan of a conv launch, as the launchers chose it (read back by pp_op_conv_last_plan, so that tests can show
+// which kernel branch a case ran).
+struct PPConvPlan {
+  char kind;     // 'g' flat GEMM kernel, 'h' TMA halo-tile kernel, 'i' cp.async implicit GEMM, 'p' recorded into a
+                 // multi-layer program, '?' none yet
+  int m;         // halo: MT (128-pixel sub-tiles per CTA tile); gemm: MB (m64 blocks per consumer warpgroup); else 0
+  int bn;        // N tile width
+  int tps;       // halo: filter taps per weight stage; else 0
+  int flat;      // halo: 1x1 flat mode (gemm: always 1)
+  int tma_out;   // fragment epilogue + TMA stores (gemm: always 1)
+  int sa, sb;    // stages of the A (patch / im2col) and B (weight) rings; igemm / gemm: one ring, sb = sa
+};
+// the plan of the last pp_launch_conv of this thread; the launchers fill it in
+PPConvPlan& pp_last_conv_plan();
+// which kernel the last pp_launch_conv of this thread went to (PPConvPlan::kind; profiling labels)
+inline char pp_last_conv_kind() { return pp_last_conv_plan().kind; }
 // conv_halo.cu: TMA halo-tile kernel for stride-1 convolutions (dispatched from pp_launch_conv when eligible).
 // `p` must already carry num_kc / vec_ok.
 int pp_conv_halo_eligible(const PPConvParams& p);

@@ -64,6 +64,9 @@ _SIGNATURES = {
     "pp_op_conv": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _F, _VP, _VP, _VP]),
     "pp_op_conv_ex": (_I, [_VP, _CP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _I, _VP, _I, _I, _VP, _I, _I, _VP,
                            _I, _I, _VP]),
+    "pp_op_conv_segs": (_I, [_VP, _CP, _I, ctypes.POINTER(_VP)] + [ctypes.POINTER(_I)] * 4 + [_I] * 12 + [_F, _F, _I, _VP,
+                             _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _I, _VP]),
+    "pp_op_conv_last_plan": (_I, [ctypes.POINTER(_I), _I]),
     "pp_op_corr_lookup": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _LL, _I, _I, _VP]),
     "pp_op_conv_tf32": (_I, [_VP, _CP, _VP, _I, _I, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I,
                              _F, _F, _I, _VP, _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _VP]),
@@ -792,6 +795,39 @@ class Engine:
             self.h, name.encode(), _ptr(x), xC, x_co, N, H, W, pad[0], pad[1], epi, act, float(slope), float(scale), act2,
             _ptr(a0), C(a0), a0_co, _ptr(a1), C(a1), a1_co, _ptr(out), C(out), out_co, self._stream()))
         return out
+
+    def op_conv_segs(self, name, segs, out, out_co=0, out_gstep=0, out_f32=False, stride=(1, 1), pad=(0, 0),
+                     dilation=(1, 1), replicate=False, act=ACT_NONE, slope=0.0, scale=1.0, act2=ACT_NONE, residual=None,
+                     gru_zr=None, gru_h=None):
+        """One fp16 convolution (weights from register_conv) built as the stages build it (pp_op_conv_segs).
+        segs: 1..6 input segments (x [N,H,W,C] fp16, first channel, channels, gstep): the layer's input is their channel
+        concatenation, group g reading each segment from channel co + g * gstep.  out [N,OH,OW,C'] fp16 written from
+        channel out_co (+ g * out_gstep), or with out_f32 float32.  Epilogue as in op_conv_ex."""
+        N, H, W = segs[0][0].shape[:3]
+        n = len(segs)
+        ints = lambda v: (ctypes.c_int * n)(*[int(i) for i in v])
+        ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t, *_ in segs])
+        C = lambda t: 0 if t is None else t.shape[-1]
+        epi, a0, a0_co, a1, a1_co = self.EPI_STD, None, 0, None, 0
+        if residual is not None:
+            a0, a0_co = residual
+        if gru_zr is not None:
+            epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_ZR, gru_zr
+        if gru_h is not None:
+            epi, (a0, a0_co, a1, a1_co) = self.EPI_GRU_H, gru_h
+        self._check(self.lib.pp_op_conv_segs(
+            self.h, name.encode(), n, ptrs, ints(t.shape[-1] for t, *_ in segs), ints(s[1] for s in segs),
+            ints(s[2] for s in segs), ints(s[3] for s in segs), N, H, W, stride[0], stride[1], pad[0], pad[1],
+            dilation[0], dilation[1], int(replicate), epi, act, float(slope), float(scale), act2, _ptr(a0), C(a0), a0_co,
+            _ptr(a1), C(a1), a1_co, _ptr(out), C(out), out_co, out_gstep, int(out_f32), self._stream()))
+        return out
+
+    def op_conv_last_plan(self) -> dict:
+        """The tile plan of this thread's last convolution launch (pp_op_conv_last_plan): kernel 'g' / 'h' / 'i' / 'p',
+        m (halo MT or gemm MB), bn, tps, flat, tma_out, sa, sb."""
+        v = (ctypes.c_int * 8)()
+        self._check(self.lib.pp_op_conv_last_plan(v, 8))
+        return dict(kernel=chr(v[0]), m=v[1], bn=v[2], tps=v[3], flat=v[4], tma_out=v[5], sa=v[6], sb=v[7])
 
     def op_corr_lookup(self, levels, coords, h8, w8):
         nq = coords.shape[0]

@@ -179,6 +179,20 @@ PP_API int pp_op_conv_ex(pp_handle h, const char* name, const void* x_f16, int x
                          int pw, int epi, int act, float slope, float scale, int act2, const void* aux0_f16, int aux0_C,
                          int aux0_co, void* aux1_f16, int aux1_C, int aux1_co, void* out_f16, int out_C, int out_co,
                          void* stream);
+/* One fp16 convolution of any layout a stage builds: nseg (1..6) input segments, segment i = channels
+ * [x_co[i], x_co[i] + x_ch[i]) of x_f16[i] [N][H][W][x_C[i]], plus g * x_gstep[i] for group g; weights registered with
+ * zero-padded input channels read the last segment zero-extended.  Stride sh x sw, padding ph x pw (zeros, or with
+ * replicate the edge pixels), dilation dh x dw.  Output out [N][OH][OW][out_C] from channel out_co (+ g * out_gstep), fp16,
+ * or with out_fp32 plain fp32.  Epilogue epi / act / slope / scale / act2 / aux0 / aux1 as in pp_op_conv_ex. */
+PP_API int pp_op_conv_segs(pp_handle h, const char* name, int nseg, const void* const* x_f16, const int* x_C,
+                           const int* x_co, const int* x_ch, const int* x_gstep, int N, int H, int W, int sh, int sw,
+                           int ph, int pw, int dh, int dw, int replicate, int epi, int act, float slope, float scale,
+                           int act2, const void* aux0_f16, int aux0_C, int aux0_co, void* aux1_f16, int aux1_C,
+                           int aux1_co, void* out, int out_C, int out_co, int out_gstep, int out_fp32, void* stream);
+/* The tile plan of the calling thread's last convolution launch, the first n of: kernel ('g' flat GEMM, 'h' halo tile,
+ * 'i' implicit GEMM, 'p' recorded into a program, '?' none), MT (halo) or MB (gemm), N tile width, filter taps per weight
+ * stage (halo), flat mode, TMA-store epilogue, patch / A stages, weight stages. */
+PP_API int pp_op_conv_last_plan(int* plan, int n);
 PP_API int pp_op_corr_lookup(pp_handle h, const void* l0, const void* l1, const void* l2, const void* l3,
                       const float* coords, void* out_f16, long long nq, int h8, int w8, void* stream);
 /* Operators of the fp32 RAFT and flow-completion paths (pp_raft_bidir_fp32, pp_flow_complete_fp32).  Split tensors are fp32 [pix][hi C | lo C] with hi = tf32(x),
