@@ -330,6 +330,13 @@ int pp_preprocess(pp_handle h, const float* image, const float* mask, int mask_f
   return PP_OK;
 }
 
+// Coefficient scratch (ints) of pp_k_resize_bicubic_u8 for an H x W -> out_h x out_w resize, both passes
+static size_t resize_coef_ints(int H, int W, int out_h, int out_w) {
+  const int mx = out_h > out_w ? out_h : out_w;
+  const double sc = fmax(fmax((double)H / out_h, (double)W / out_w), 1.0);
+  return 2 * (size_t)mx * ((size_t)ceil(2.0 * sc) * 2 + 1 + 2) + 64;
+}
+
 // Shared tail of the pre-processing entry points: 8-bit frames / masks at the input size -> outputs at the processing size
 static int preprocess_from_u8(PPEngine& e, const uint8_t* u8_in, const uint8_t* m_in, int mask_frames, int T, int H, int W,
                               int out_h, int out_w, int flow_mask_dilates, int mask_dilates, uint8_t* orig_u8, float* frames,
@@ -340,9 +347,7 @@ static int preprocess_from_u8(PPEngine& e, const uint8_t* u8_in, const uint8_t* 
     const size_t mid_px = (size_t)T * H * out_w;
     uint8_t *tmp, *m_out;
     int* coef;
-    const int mx = out_h > out_w ? out_h : out_w;
-    const double sc = fmax(fmax((double)H / out_h, (double)W / out_w), 1.0);
-    const size_t coef_ints = 2 * (size_t)mx * ((size_t)ceil(2.0 * sc) * 2 + 1 + 2) + 64;
+    const size_t coef_ints = resize_coef_ints(H, W, out_h, out_w);
     PP_TRY(pp_alloc(e, &tmp, mid_px * 3, "resize pass 1"));
     PP_TRY(pp_alloc(e, &m_out, (size_t)mask_frames * out_h * out_w, "mask resized"));
     PP_TRY(pp_alloc(e, &coef, coef_ints, "resize coefficients"));
@@ -393,6 +398,33 @@ int pp_preprocess_u8(pp_handle h, const uint8_t* image_u8, const uint8_t* mask_u
                             orig_u8, frames, flow_masks, masks_dilated, as_stream(stream));
 }
 
+int pp_preprocess_outpaint_u8(pp_handle h, const uint8_t* image_u8, int T, int H, int W, int rw, int rh, int pw, int ph,
+                              uint8_t* orig_u8, float* frames, float* flow_masks, float* masks_dilated, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(image_u8 && orig_u8 && frames && flow_masks && masks_dilated, "pp_preprocess_outpaint_u8: null pointer");
+  PP_REQUIRE(T > 0 && H > 0 && W > 0 && rw > 0 && rh > 0, "pp_preprocess_outpaint_u8: bad size (T %d, %dx%d -> %dx%d)", T,
+             W, H, rw, rh);
+  PP_REQUIRE(rw <= pw && rh <= ph, "pp_preprocess_outpaint_u8: the %dx%d frames do not fit the %dx%d canvas", rw, rh, pw,
+             ph);
+  ArenaGuard guard(e.arena);
+  cudaStream_t st = as_stream(stream);
+  const uint8_t* window = image_u8;
+  if (rw != W || rh != H) {   // PIL's bicubic resize of the 8-bit frames to the processing size (image_utils.py:98-103)
+    uint8_t *tmp, *resized;
+    int* coef;
+    const size_t coef_ints = resize_coef_ints(H, W, rh, rw);
+    PP_TRY(pp_alloc(e, &tmp, (size_t)T * H * rw * 3, "resize pass 1"));
+    PP_TRY(pp_alloc(e, &resized, (size_t)T * rh * rw * 3, "outpaint window"));
+    PP_TRY(pp_alloc(e, &coef, coef_ints, "resize coefficients"));
+    PP_TRY(pp_k_resize_bicubic_u8(image_u8, resized, tmp, coef, coef_ints, T, H, W, 3, rh, rw, st));
+    window = resized;
+    e.launches += (rw != W) + (rh != H);
+  }
+  PP_TRY(pp_k_outpaint_canvas(window, T, rw, rh, pw, ph, orig_u8, frames, flow_masks, masks_dilated, st));
+  e.launches++;
+  return PP_OK;
+}
+
 // Host helper (no GPU involved): float [0,1] -> uint8 with the reference's arithmetic -- x * 255 in float32, clip to
 // [0, 255], truncate (utils/image_utils.py:106-114, 128-134) -- on `threads` host threads.  Lets a host caller ship 1/4 of
 // the bytes over PCIe: quantise straight into a page-locked staging buffer, copy, then pp_preprocess_u8.
@@ -416,6 +448,14 @@ int pp_host_quantize_u8(const float* src, uint8_t* dst, long long n, int threads
   }
   for (auto& th : pool) th.join();
   return PP_OK;
+}
+
+int pp_quantize_u8(pp_handle h, const float* src, uint8_t* dst, long long n, void* stream) {
+  PP_HANDLE(h);
+  PP_REQUIRE(src && dst && n >= 0, "pp_quantize_u8: bad argument");
+  if (n == 0) return PP_OK;
+  e.launches++;
+  return pp_k_quantize_u8(src, dst, n, as_stream(stream));
 }
 
 int pp_postprocess(pp_handle h, const uint8_t* comp_u8, float* image_out, long long n, void* stream) {

@@ -118,3 +118,5 @@ int pp_k_quantize_u8(const float* img, uint8_t* u8, long long n, cudaStream_t st
 int pp_k_u8_to_frames(const uint8_t* u8, float* frames, int T, int H, int W, cudaStream_t st);
 int pp_k_dilate_masks_u8(const uint8_t* mask_u8, int Tm, int T, int H, int W, int iters_flow, int iters_dil,
                          float* flow_masks, float* masks_dilated, cudaStream_t st);
+int pp_k_outpaint_canvas(const uint8_t* window, int T, int rw, int rh, int pw, int ph, uint8_t* orig, float* frames,
+                         float* flow_masks, float* masks_dilated, cudaStream_t st);

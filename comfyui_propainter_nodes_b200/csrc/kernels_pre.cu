@@ -1,6 +1,5 @@
 // Device-side pre/post-processing with the reference's integer semantics (SURVEY.md section 8f.1; reference
-// utils/image_utils.py:106-197, 276-290).  Used when no resize is needed (input size == processing size);
-// resizing goes through PIL on the host so the bicubic filter stays bit-identical.
+// utils/image_utils.py:106-290) for both nodes, bit-identical to the host path, PIL's 8-bit bicubic resize included.
 #include <math.h>
 
 #include <vector>
@@ -11,6 +10,12 @@ namespace {
 
 constexpr int TPB = 256;
 inline int nblocks(long long n, int per = TPB) { return (int)((n + per - 1) / per); }
+
+// 8-bit value -> frame value in [-1,1]: float32 u8 / 255, * 2, - 1, each rounded to nearest like the host's
+// _stack_to_tensor(...) * 2 - 1 (image_utils.py:95-103); explicit roundings, so --use_fast_math cannot change them
+__device__ __forceinline__ float u8_to_pm1(uint8_t q) {
+  return __fsub_rn(__fmul_rn(__fdiv_rn((float)q, 255.f), 2.f), 1.f);
+}
 
 // IMAGE [T,H,W,3] float 0..1 -> uint8 by *255, clip, truncate (image_utils.py:112) and
 // frames [T,3,H,W] = u8/255*2-1 (image_utils.py:186-190)
@@ -24,7 +29,7 @@ __global__ void quantize_frames(const float* __restrict__ img, uint8_t* __restri
     const float v = fminf(fmaxf(__fmul_rn(img[idx * 3 + c], 255.f), 0.f), 255.f);
     const uint8_t q = (uint8_t)(int)v;
     u8[idx * 3 + c] = q;
-    frames[(t * 3 + c) * HW + p] = __fsub_rn(__fmul_rn(__fdiv_rn((float)q, 255.f), 2.f), 1.f);
+    frames[(t * 3 + c) * HW + p] = u8_to_pm1(q);
   }
 }
 
@@ -99,7 +104,29 @@ __global__ void u8_to_frames(const uint8_t* __restrict__ u8, float* __restrict__
   const long long t = idx / HW, p = idx - t * HW;
 #pragma unroll
   for (int c = 0; c < 3; ++c)
-    frames[(t * 3 + c) * HW + p] = __fsub_rn(__fmul_rn(__fdiv_rn((float)u8[idx * 3 + c], 255.f), 2.f), 1.f);
+    frames[(t * 3 + c) * HW + p] = u8_to_pm1(u8[idx * 3 + c]);
+}
+
+// Outpainting canvas (extrapolation + _tensorise, image_utils.py:115-139): the rw x rh frames src [T,rh,rw,3] placed at
+// (x0, y0) on a zero pw x ph canvas -> orig [T,ph,pw,3], frames [T,3,ph,pw] = u8/255*2-1, and the band masks [T,1,ph,pw]
+// in {0,1}: masks_dilated is 1 outside the window, flow_masks also on the window's outer iw columns / ih rows.
+__global__ void outpaint_canvas(const uint8_t* __restrict__ src, uint8_t* __restrict__ orig, float* __restrict__ frames,
+                                float* __restrict__ flow_masks, float* __restrict__ masks_dilated, int rw, int rh, int pw,
+                                int ph, int x0, int y0, int iw, int ih, long long total) {
+  const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;  // over T*ph*pw pixels
+  if (idx >= total) return;
+  const long long HW = (long long)ph * pw, t = idx / HW, p = idx - t * HW;
+  const int sy = (int)(p / pw) - y0, sx = (int)(p % pw) - x0;
+  const bool in = sx >= 0 && sx < rw && sy >= 0 && sy < rh;
+  const bool inner = sx >= iw && sx < rw - iw && sy >= ih && sy < rh - ih;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const uint8_t q = in ? src[((t * rh + sy) * rw + sx) * 3 + c] : 0;
+    orig[idx * 3 + c] = q;
+    frames[(t * 3 + c) * HW + p] = u8_to_pm1(q);
+  }
+  flow_masks[idx] = inner ? 0.f : 1.f;
+  masks_dilated[idx] = in ? 0.f : 1.f;
 }
 
 // uint8 [T,H,W,3] -> float32 / 255 (handle_output, image_utils.py:281-283)
@@ -221,6 +248,20 @@ int pp_k_dilate_masks_u8(const uint8_t* mask_u8, int Tm, int T, int H, int W, in
   PP_REQUIRE(Tm == 1 || Tm == T, "prepare_masks: mask length %d must be 1 or %d", Tm, T);
   dilate_diamond<<<nblocks((long long)T * H * W), TPB, 0, st>>>(mask_u8, flow_masks, Tm, T, H, W, iters_flow);
   dilate_diamond<<<nblocks((long long)T * H * W), TPB, 0, st>>>(mask_u8, masks_dilated, Tm, T, H, W, iters_dil);
+  PP_CUDA_CHECK(cudaGetLastError());
+  return PP_OK;
+}
+
+// window [T,rh,rw,3] uint8 (0 < rw <= pw, 0 < rh <= ph) centred on the pw x ph canvas like extrapolation
+// (image_utils.py:120-130): offsets int((pw - rw) / 2), int((ph - rh) / 2); the flow mask's 4-px inset only on the axes
+// whose band is wider than 10 px
+int pp_k_outpaint_canvas(const uint8_t* window, int T, int rw, int rh, int pw, int ph, uint8_t* orig, float* frames,
+                         float* flow_masks, float* masks_dilated, cudaStream_t st) {
+  const int x0 = (pw - rw) / 2, y0 = (ph - rh) / 2;
+  const int iw = x0 > 10 ? 4 : 0, ih = y0 > 10 ? 4 : 0;
+  const long long total = (long long)T * ph * pw;
+  outpaint_canvas<<<nblocks(total), TPB, 0, st>>>(window, orig, frames, flow_masks, masks_dilated, rw, rh, pw, ph, x0, y0,
+                                                  iw, ih, total);
   PP_CUDA_CHECK(cudaGetLastError());
   return PP_OK;
 }

@@ -56,6 +56,8 @@ _SIGNATURES = {
     "pp_preprocess_resize": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
     "pp_preprocess_u8": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
     "pp_host_quantize_u8": (_I, [_VP, _VP, _LL, _I]),
+    "pp_quantize_u8": (_I, [_VP, _VP, _VP, _LL, _VP]),
+    "pp_preprocess_outpaint_u8": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
     "pp_postprocess": (_I, [_VP, _VP, _VP, _LL, _VP]),
     "pp_launch_count": (_LL, [_VP]),
     "pp_workspace_peak": (_SZ, [_VP]),
@@ -688,17 +690,7 @@ class Engine:
 
     def _preprocess_host(self, image, mask, flow_mask_dilates, mask_dilates, ow, oh):
         T, H, W, _ = image.shape
-        threads = min(os.cpu_count() or 1, int(os.environ.get("PP_HOST_THREADS", 16)))
-        try:
-            img8 = torch.empty(image.shape, dtype=torch.uint8, pin_memory=True)
-            msk8 = torch.empty(mask.shape, dtype=torch.uint8, pin_memory=True)
-        except RuntimeError:        # locked-memory limit: pageable staging still moves 1/4 of the bytes
-            img8 = torch.empty(image.shape, dtype=torch.uint8)
-            msk8 = torch.empty(mask.shape, dtype=torch.uint8)
-        self._check(self.lib.pp_host_quantize_u8(_ptr(image), _ptr(img8), image.numel(), threads))
-        img8d = img8.to(self.device, non_blocking=True)
-        self._check(self.lib.pp_host_quantize_u8(_ptr(mask), _ptr(msk8), mask.numel(), threads))
-        msk8d = msk8.to(self.device, non_blocking=True)
+        (img8d, img8), (msk8d, msk8) = self._upload_u8(image), self._upload_u8(mask)
         orig = torch.empty(T, oh, ow, 3, device=self.device, dtype=torch.uint8)
         frames = torch.empty(T, 3, oh, ow, device=self.device, dtype=torch.float32)
         fm = torch.empty(T, 1, oh, ow, device=self.device, dtype=torch.float32)
@@ -707,6 +699,43 @@ class Engine:
                                               int(flow_mask_dilates), int(mask_dilates), _ptr(orig), _ptr(frames), _ptr(fm),
                                               _ptr(md), self._stream()))
         self._keep_staging = (img8, msk8)      # the async copies read them; released at the next call
+        return frames.unsqueeze(0), fm.unsqueeze(0), md.unsqueeze(0), orig
+
+    def _upload_u8(self, x):
+        """Contiguous float32 host tensor -> (uint8 device tensor, host staging): the reference's truncation on the host
+        cores (pp_host_quantize_u8) straight into page-locked staging, then an asynchronous copy of 1/4 of the bytes.  The
+        caller keeps the staging tensor alive until the copy has run."""
+        threads = min(os.cpu_count() or 1, int(os.environ.get("PP_HOST_THREADS", 16)))
+        try:
+            x8 = torch.empty(x.shape, dtype=torch.uint8, pin_memory=True)
+        except RuntimeError:        # locked-memory limit: pageable staging still moves 1/4 of the bytes
+            x8 = torch.empty(x.shape, dtype=torch.uint8)
+        self._check(self.lib.pp_host_quantize_u8(_ptr(x), _ptr(x8), x.numel(), threads))
+        return x8.to(self.device, non_blocking=True), x8
+
+    def preprocess_outpaint(self, image, icfg):
+        """Device version of convert_image_to_frames + extrapolation + prepare_frames_and_masks_for_outpaint (reference
+        utils/image_utils.py:98-116, 178-252), bit for bit: the frames, resized to ``icfg.process_size`` when that is not
+        their size (PIL's 8-bit bicubic resampler), centred on a zero canvas of ``icfg.outpaint_size`` with the band
+        masks around them.  image [T,H,W,3] float 0..1 (host or device).
+        -> frames [1,T,3,ph,pw], flow_masks [1,T,1,ph,pw], masks_dilated [1,T,1,ph,pw] (float32), originals uint8
+        [T,ph,pw,3], all on the device."""
+        T, H, W, _ = image.shape
+        rw, rh = (int(v) for v in icfg.process_size)
+        pw, ph = (int(v) for v in icfg.outpaint_size)
+        if image.device.type == "cpu" and image.dtype == torch.float32:
+            img8d, staging = self._upload_u8(image.contiguous())        # as in preprocess: 1/4 of the bytes over PCIe
+        else:
+            img = image.to(self.device, torch.float32, non_blocking=True).contiguous()
+            img8d, staging = torch.empty(img.shape, device=self.device, dtype=torch.uint8), None
+            self._check(self.lib.pp_quantize_u8(self.h, _ptr(img), _ptr(img8d), img.numel(), self._stream()))
+        orig = torch.empty(T, ph, pw, 3, device=self.device, dtype=torch.uint8)
+        frames = torch.empty(T, 3, ph, pw, device=self.device, dtype=torch.float32)
+        fm = torch.empty(T, 1, ph, pw, device=self.device, dtype=torch.float32)
+        md = torch.empty_like(fm)
+        self._check(self.lib.pp_preprocess_outpaint_u8(self.h, _ptr(img8d), T, H, W, rw, rh, pw, ph, _ptr(orig),
+                                                       _ptr(frames), _ptr(fm), _ptr(md), self._stream()))
+        self._keep_staging = staging
         return frames.unsqueeze(0), fm.unsqueeze(0), md.unsqueeze(0), orig
 
     def postprocess(self, comp_u8: torch.Tensor) -> torch.Tensor:

@@ -39,6 +39,22 @@ def check_inputs(frames: torch.Tensor, masks: torch.Tensor) -> None:
                         f" Mask: ({masks.size(dim=1)}, {masks.size(dim=2)})")
 
 
+def check_outpaint_sizes(icfg: iu.ImageOutpaintConfig, n: int) -> None:
+    """The Outpaint node's input checks.  The reference performs none, and its pre-processing fails in PIL, numpy or
+    torch instead; these raise the same exception types, before any model is loaded.  With a resize: an empty clip
+    IndexError, a processing size of zero or a canvas smaller than the frames ValueError.  Without one: RuntimeError."""
+    (rw, rh), (pw, ph) = icfg.process_size, icfg.outpaint_size
+    resize = tuple(icfg.process_size) != tuple(icfg.input_size)
+    if n == 0:
+        raise (IndexError if resize else RuntimeError)("Outpainting needs at least one frame")
+    if resize and (rw <= 0 or rh <= 0):
+        raise ValueError(f"height and width must be > 0, but the processing size is {rw}x{rh}")
+    if pw < rw or ph < rh:
+        raise (ValueError if resize else RuntimeError)(
+            f"The {rw}x{rh} frames do not fit the {pw}x{ph} outpainting canvas: width_scale and height_scale must not "
+            "shrink it below the processing size")
+
+
 def _int(default, lo, hi):
     return ("INT", {"default": default, "min": lo, "max": hi})
 
@@ -153,14 +169,14 @@ class ProPainterOutpaint:
                                       width_scale, height_scale)
         cfg = ProPainterConfig(ref_stride, neighbor_length, subvideo_length, raft_iter, fp16, n, device,
                                icfg.outpaint_size)
-        if tuple(icfg.process_size) == tuple(input_size):
-            # no resize: canvas and band masks are assembled on the device (same integer semantics)
-            ft, fm, md, orig = iu.outpaint_tensors(image, icfg, device)
-        else:
-            canvas, flow_masks, masks_dilated = iu.extrapolation(iu.convert_image_to_frames(image), icfg)
-            ft, fm, md, originals = iu.prepare_frames_and_masks_for_outpaint(canvas, flow_masks, masks_dilated, device)
-            orig = torch.from_numpy(np.stack(originals))
+        check_outpaint_sizes(icfg, n)
         models = initialize_models(cfg.device, cfg.fp16)
+        # quantisation, PIL's 8-bit bicubic resize, the canvas and its band masks run on the device with the reference's
+        # integer semantics, bit for bit
+        eng = models.raft_model.engine
+        pw, ph = icfg.outpaint_size
+        eng.reserve_for_clip(n, ph, pw)
+        ft, fm, md, orig = eng.preprocess_outpaint(image, icfg)
         images, out_masks, _ = _run(models, ft, fm, md, orig, cfg)
         out_w, out_h = cfg.process_size
         return images, out_masks, out_w, out_h

@@ -154,6 +154,18 @@ PP_API int pp_preprocess_u8(pp_handle h, const uint8_t* image_u8, const uint8_t*
 /* HOST helper, no GPU work: dst[i] = (uint8)trunc(clip(src[i] * 255, 0, 255)) in float32, the reference's conversion
  * (utils/image_utils.py:106-114, 128-134), on `threads` host threads; src / dst are host pointers. */
 PP_API int pp_host_quantize_u8(const float* src, uint8_t* dst, long long n, int threads);
+/* The same conversion on the device, for an IMAGE that is already there: src float, dst uint8, n elements. */
+PP_API int pp_quantize_u8(pp_handle h, const float* src, uint8_t* dst, long long n, void* stream);
+/* Device pre-processing of the Outpaint node (reference utils/image_utils.py:98-116, 178-252: convert_image_to_frames,
+ * extrapolation, prepare_frames_and_masks_for_outpaint) from 8-bit frames image_u8 [T,H,W,3]: resized to rw x rh
+ * when that differs from W x H (PIL's 8-bit bicubic resampler, bit for bit, as in pp_preprocess_resize), placed at
+ * (int((pw - rw) / 2), int((ph - rh) / 2)) on a zero pw x ph canvas -> orig_u8 [T,ph,pw,3], frames [T,3,ph,pw] in
+ * [-1,1], and the band masks [T,1,ph,pw] in {0,1}: masks_dilated is 1 outside the frames, flow_masks is that band
+ * plus a 4-px inset into the frames on each axis whose band is wider than 10 px.  Requires 0 < rw <= pw, 0 < rh <= ph.
+ * All device pointers. */
+PP_API int pp_preprocess_outpaint_u8(pp_handle h, const uint8_t* image_u8, int T, int H, int W, int rw, int rh, int pw,
+                                     int ph, uint8_t* orig_u8, float* frames, float* flow_masks, float* masks_dilated,
+                                     void* stream);
 /* uint8 frames -> float32 / 255 (reference handle_output, utils/image_utils.py:276-290). */
 PP_API int pp_postprocess(pp_handle h, const uint8_t* comp_u8, float* image_out, long long n, void* stream);
 
